@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the predictor–corrector sampling hot path (BASELINE.json metric).
+"""Benchmark of the predictor–corrector sampling hot path.
 
 Metric: PC-sampler images/sec, NCSN++ cont. CIFAR-10, VE-SDE, 1000 steps
 (``configs/ve/cifar10_ncsnpp_continuous.py`` with ``model.init_scale = 1``, random-init
@@ -32,8 +32,8 @@ import torch
 REPO = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, REPO)
 
-ALG_FLOP_PER_IMG_STEP = 43.58e9      # SURVEY.md §8(d): 2 evals x 21.788 GFLOP (2*MAC), measured on the reference
-ALG_BYTES_PER_IMG_STEP = 153.9e6     # SURVEY.md §8(d): fp32 contraction operands only, everything else fused
+ALG_FLOP_PER_IMG_STEP = 43.58e9      # 2 evals x 21.788 GFLOP (2*MAC), counted on the reference network
+ALG_BYTES_PER_IMG_STEP = 153.9e6     # fp32 contraction operands only, everything else fused
 N_SAMPLER_STEPS = 1000
 
 
@@ -44,11 +44,12 @@ def load_peaks():
       d = json.load(fh)
     return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'], bf16_tflops_sustained=d['bf16_tflops_sustained'],
                 source='measured (MEASURED_PEAKS.json)')
-  return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+  # NVIDIA's H100 SXM data sheet (dense, 700 W card); it states no sustained rate, so the burst figure stands in for it
+  return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source='fallback (H100 SXM data sheet)')
 
 
 class ClockSampler:
-  """nvidia-smi clocks/throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks/throttle reasons sampled during the timed region."""
 
   def __init__(self, index):
     self.index, self.rows, self.proc = index, [], None
@@ -83,21 +84,18 @@ class ClockSampler:
                 reasons=sorted(reasons), samples=len(sm))
 
 
-SEPARATE_GROUPNORM_DEFAULT = True   # the plan bench.py measures by default = the package default (the faster one in the same-run A/B; both are in `variants`)
-
-
 def headline_config():
   from score_sde_pytorch_b200 import configs
   cfg = configs.ve_cifar10_ncsnpp_continuous()
-  cfg.model.init_scale = 1.0          # BASELINE.md §2: init_scale=0 zeroes every block's last conv
+  cfg.model.init_scale = 1.0          # init_scale=0 would zero every block's last conv
   return cfg
 
 
 # ----------------------------------------------------------------------------------------------
-# CPU arm: the UNMODIFIED reference (baseline/_ref, installed by tools/install_ref.sh) on the host cores
+# CPU arm: the UNMODIFIED reference (oracle/_ref, installed by oracle/install_ref.sh) on the host cores
 # ----------------------------------------------------------------------------------------------
-REF_DIR = os.path.join(REPO, 'baseline', '_ref')
-REF_EXT_DIR = os.path.join(REPO, 'baseline', '_ref_ext')
+REF_DIR = os.path.join(REPO, 'oracle', '_ref')
+REF_EXT_DIR = os.path.join(REF_DIR, '_ext')
 
 
 def physical_cores():
@@ -123,12 +121,12 @@ def physical_cores():
 
 
 def import_reference():
-  """Import the reference's own modules from baseline/_ref (never from /root/reference: that path does not exist on
-  the GPU box).  `ml_collections` is not installed: its ConfigDict is only used as an attribute dict by the
-  reference's config files, so a 6-line stand-in is injected into sys.modules.  Returns the module namespace."""
+  """Import the reference's own modules from the copy under oracle/_ref.  `ml_collections` is not installed: its
+  ConfigDict is only used as an attribute dict by the reference's config files, so a 6-line stand-in is injected into
+  sys.modules.  Returns the module namespace."""
   import types
   if not os.path.isdir(REF_DIR):
-    raise FileNotFoundError(f'{REF_DIR} missing: run tools/install_ref.sh where /root/reference exists')
+    raise FileNotFoundError(f'{REF_DIR} missing: run oracle/install_ref.sh REFERENCE_CHECKOUT')
   if 'ml_collections' not in sys.modules:
     class ConfigDict(dict):
       def __getattr__(self, k):
@@ -141,7 +139,7 @@ def import_reference():
     m.ConfigDict = ConfigDict
     sys.modules['ml_collections'] = m
   os.environ.setdefault('TORCH_EXTENSIONS_DIR', REF_EXT_DIR)      # the two JIT extensions of op/ were pre-built there
-  os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '10.0')
+  os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '9.0')
   # our own package has modules of the same names (sampling, sde_lib, ...) under score_sde_pytorch_b200/, never
   # top-level, so putting the reference first on sys.path shadows nothing of ours
   if REF_DIR not in sys.path:
@@ -187,7 +185,7 @@ def reference_pc_steps(batch, steps, warmup):
 
 
 def port_pc_steps(batch, steps, warmup):
-  """Fallback when baseline/_ref is absent: the oracle port (plain PyTorch fp32 restatement of the same path)."""
+  """Fallback when oracle/_ref is absent: the oracle port (plain PyTorch fp32 restatement of the same path)."""
   from oracle import ncsnpp_oracle as NO
   from oracle import sampling_oracle as SO
   from score_sde_pytorch_b200.models.ncsnpp import NCSNpp
@@ -223,8 +221,8 @@ def cpu_pc_steps(batch, steps, warmup):
     times, kind = port_pc_steps(batch, steps, warmup)
   t_med, t_mean = float(np.median(times)), float(np.mean(times))
   spread = (max(times) - min(times)) / t_med if len(times) > 1 else 0.0
-  what = ("the reference's own NCSNpp + shared_corrector_update_fn/shared_predictor_update_fn (baseline/_ref, unmodified)"
-          if kind == 'reference' else 'the oracle port (baseline/_ref absent)')
+  what = ("the reference's own NCSNpp + shared_corrector_update_fn/shared_predictor_update_fn (oracle/_ref, unmodified)"
+          if kind == 'reference' else 'the oracle port (oracle/_ref absent)')
   return dict(value=batch / (N_SAMPLER_STEPS * t_med), unit='images/s', cores=threads, kind=kind,
               sample=f'{steps} PC iterations (2 network evals each) of {what} at batch {batch} after {warmup} warm-up; '
                      f'median {t_med:.3f} s/iteration (mean {t_mean:.3f}, spread {spread:.1%}), extrapolated to '
@@ -267,7 +265,7 @@ def run_reference_arm(args):
     # thread count and binding must be in the environment before libgomp starts: re-exec once
     os.execve(sys.executable, [sys.executable] + sys.argv, pinned_env())
   batch = args.cpu_batch
-  steps = max(args.steps, 5)                 # >= 5 timed iterations: the median is the reported figure
+  steps = args.steps
   r = cpu_pc_steps(batch, steps, max(args.warmup, 1))
   line = dict(impl='reference', metric='PC-sampler images/sec, NCSN++ CIFAR-10 1000-step VE', value=r['value'],
               unit='images/s', n_gpus=args.gpus, steps=steps, warmup=max(args.warmup, 1), ms_per_step=r['ms_per_step'],
@@ -284,23 +282,9 @@ def run_reference_arm(args):
 # ----------------------------------------------------------------------------------------------
 # GPU arm
 # ----------------------------------------------------------------------------------------------
-def load_traffic(precision):
-  """DRAM bytes per launch of the contraction kernels from the committed ncu metrics pass of one PC step
-  (profiles/traffic_<precision>.json, written by tools/summarize_traffic.py); None when no capture is committed."""
-  path = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', f'traffic_{precision}.json')
-  try:
-    k = json.load(open(path))['kernels']
-    for name, d in k.items():
-      if name.startswith('tcgen05'):
-        return round(d['dram_bytes_per_launch'])
-  except (OSError, KeyError, ValueError):
-    pass
-  return None
-
-
 def measure_tf32_peak(dev, f16=False):
-  """cuBLAS GEMM throughput on this device in the operand format the engine computes in: TF32 (kind::tf32
-  work) or fp16 with fp32 accumulation (kind::f16 work) - the measured denominator of the tensor roofline."""
+  """cuBLAS GEMM throughput on this device in the operand format the engine computes in: TF32 or fp16 with fp32
+  accumulation - a measured comparison for the tensor roofline (the engine itself never calls cuBLAS)."""
   n = 8192
   a = torch.randn(n, n, device=dev)
   b = torch.randn(n, n, device=dev)
@@ -381,10 +365,11 @@ def profile_kinds(model, B, dev, x0):
   return eng, ms_k, fl_k, n_k
 
 
-def underfilled_launches(model, B, dev, x0, sms=148):
+def underfilled_launches(model, B, dev, x0):
   """Strong-scaling diagnosis: per-op time at this batch and which contraction launches have fewer tiles than SMs."""
   import ctypes
   from score_sde_pytorch_b200 import _lib
+  sms = torch.cuda.get_device_properties(dev).multi_processor_count
   eng = model.engine(B, dev)
   n = int(_lib.load().b200_ncsnpp_num_ops(eng['h']))
   ms = (ctypes.c_float * n)()
@@ -401,19 +386,40 @@ def underfilled_launches(model, B, dev, x0, sms=148):
   for k, r in sorted(rows.items(), key=lambda kv: -kv[1]['ms']):
     if r['kind'] != 0:
       continue
-    # tiles of a launch: M = B*H*W pixels over 128- (single), 256- (pair / swap) pixel tiles
+    # tiles of a launch: M = B*H*W pixels over 128- (single) or 256- (swap) pixel tiles
     import re
     m = re.search(r'@(\d+)', k)
     if not m:
       continue
     res = int(m.group(1))
     px_per_tile = 128 if 'single' in k else 256
-    ctas = B * res * res // px_per_tile * (2 if 'pair' in k else 1)
+    ctas = B * res * res // px_per_tile
     if 'single128' in k:
       ctas *= 2
     out_rows.append(dict(op=k, launches=r['launches'], ms=round(r['ms'], 4), ctas=ctas, fills_sms=bool(ctas >= sms),
                          tflops=round(r['flops'] / max(r['ms'], 1e-9) / 1e9, 1)))
   return out_rows
+
+
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, **arrays):
+  """Write what the timed path returned in its last step (the sampler state x and its noise-free mean x_mean, what a
+  caller of plan.run receives) as float32 .npy files, so that two builds can be compared output for output.  Inputs are
+  seeded, so the same arguments give the same inputs.  At most 64 MB in all: above that, the same fixed, seeded subset
+  of images (sorted indices from numpy's default_rng(0)) is taken from every array.  Under torch.distributed only rank
+  0 writes, so the files hold rank 0's shard of the chains."""
+  os.makedirs(out_dir, exist_ok=True)
+  host = {name: t.detach().float().cpu().numpy() for name, t in arrays.items()}
+  total = sum(a.nbytes for a in host.values())
+  if total > DUMP_CAP_BYTES:
+    n = next(iter(host.values())).shape[0]
+    keep = max(1, int(n * DUMP_CAP_BYTES // total))
+    idx = np.sort(np.random.default_rng(0).choice(n, size=keep, replace=False))
+    host = {name: a[idx] for name, a in host.items()}
+  for name, a in host.items():
+    np.save(os.path.join(out_dir, f'{name}.npy'), a)
 
 
 def run_gpu_arm(args):
@@ -438,7 +444,7 @@ def run_gpu_arm(args):
   B = args.batch if args.scaling == 'weak' else max(1, args.batch // world)
   shape = (B, 3, 32, 32)
   torch.manual_seed(0)                       # same random-init weights on every rank ...
-  model = NCSNpp(cfg, precision=args.precision, separate_groupnorm=args.separate_groupnorm).to(dev)
+  model = NCSNpp(cfg, precision=args.precision).to(dev)
   if world > 1:                              # ... and broadcast once over NCCL/NVLink anyway (the production path)
     from score_sde_pytorch_b200 import distributed as bdist
     bdist.broadcast_parameters(model, src=0)
@@ -452,7 +458,7 @@ def run_gpu_arm(args):
   x_host = sde.prior_sampling(shape).pin_memory()
   out_host = torch.empty(shape).pin_memory()
 
-  # ---- parity at the measured configuration (SURVEY 8d): K PC iterations at the full batch through the engine's
+  # ---- parity at the measured configuration: K PC iterations at the full batch through the engine's
   # plan and through the strict-fp32 GPU oracle, same prior draw, same CUDA noise stream.  The oracle is the checker
   # here, never the thing timed.  Runs on rank 0 only, before any timing; the run FAILS above the north-star bound.
   parity = None
@@ -482,6 +488,8 @@ def run_gpu_arm(args):
   clk = clocks.stop()
   ms = e0.elapsed_time(e1)
   finite = bool(torch.isfinite(x_mean).all().item())
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, x=x, x_mean=x_mean)   # before the e2e loop below reuses the plan's buffers
 
   # ---- end to end through the public plan API with host buffers, copies inside the timed region ----
   e2e_steps = args.steps
@@ -517,7 +525,7 @@ def run_gpu_arm(args):
       if kind_c.value == 0:
         _lib.call('b200_ncsnpp_op_bytes', eng['h'], i, ctypes.byref(bytes_c))
         tc_alg_bytes += bytes_c.value
-    kinds = ['tcgen05_contraction', 'cuda_core_contraction', 'groupnorm', 'fir', 'softmax', 'time_embedding', 'misc', 'mma_sync_contraction']
+    kinds = ['tensor_core_contraction', 'cuda_core_contraction', 'groupnorm', 'fir', 'softmax', 'time_embedding', 'misc', 'mma_sync_contraction']
     by_kind = {k: dict(ms=round(ms_k[i], 4), gflop=round(fl_k[i] / 1e9, 2), launches=int(n_k[i])) for i, k in enumerate(kinds)}
     fwd_ms = sum(ms_k[i] for i in range(8))
     tc_ms, tc_flops, tc_n = ms_k[0], fl_k[0], max(int(n_k[0]), 1)
@@ -530,7 +538,7 @@ def run_gpu_arm(args):
     # step is a long back-to-back run -> the SUSTAINED peak for step_tensor_fraction.  TF32 runs at half those rates.
     rate = 1.0 if f16 else 0.5
     burst, sustained = peaks['bf16_tflops'] * rate, peaks['bf16_tflops_sustained'] * rate
-    roofline = dict(bound='tensor', kernel=f"gemm_tc_kernel / gemm_tc2_kernel (tcgen05 kind::{'f16' if f16 else 'tf32'} implicit GEMM)",
+    roofline = dict(bound='tensor', kernel=f"gemm_tc_kernel (wgmma .{'f16' if f16 else 'tf32'} implicit GEMM)",
                     achieved=round(achieved, 2), peak=round(burst, 2), unit='TFLOP/s',
                     frac=round(achieved / burst, 4),
                     peak_source=(f"{peaks['source']}: bf16 burst {peaks['bf16_tflops']} TF/s" + ('' if f16 else ' x 0.5 (TF32 rate)')),
@@ -538,7 +546,7 @@ def run_gpu_arm(args):
                     cublas_in_run=round(tf32_peak, 2), frac_of_cublas_in_run=round(achieved / tf32_peak, 4) if tf32_peak else None,
                     alg_flop_per_launch=tc_flops / tc_n, avg_launch_ms=tc_ms / tc_n, launches_per_forward=tc_n,
                     kernel_share_of_forward=round(tc_ms / fwd_ms, 4) if fwd_ms else None,
-                    traffic=load_traffic(args.precision), alg_hbm_bytes_per_launch=round(tc_alg_bytes / tc_n),
+                    alg_hbm_bytes_per_launch=round(tc_alg_bytes / tc_n),
                     hbm_fraction_of_step=round(t_hbm_ms / ms_per_step, 4),
                     step_tensor_fraction=round((ALG_FLOP_PER_IMG_STEP * B / (sustained * 1e12) * 1e3) / ms_per_step, 4),
                     step_tflops=round(ALG_FLOP_PER_IMG_STEP * B / (ms_per_step * 1e-3) / 1e12, 1),
@@ -556,20 +564,9 @@ def run_gpu_arm(args):
       variants = {other: dict(value=round(B / (N_SAMPLER_STEPS * ms2 * 1e-3), 4), unit='images/s', ms_per_step=round(ms2, 4))}
       del plan2, model2
       if args.precision == 'f16':
-        # A/B of the two GroupNorm plans in the same run, on the same box (the separate streaming pass of round 1 vs
-        # GroupNorm applied on load by the consuming convolution): whichever is not the headline plan is timed here
-        torch.manual_seed(0)
-        model3 = NCSNpp(cfg, precision='f16', separate_groupnorm=not args.separate_groupnorm).to(dev)
-        plan3 = native.match_pc_plan(sde=sde, model=model3, predictor=sampling.ReverseDiffusionPredictor,
-                                     corrector=sampling.LangevinCorrector, shape=shape, snr=cfg.sampling.snr, n_steps=1,
-                                     probability_flow=False, continuous=True, eps=1e-5, device=dev)
-        ms3 = timed_steps(plan3, x_host.to(dev), args.warmup, args.steps)
-        variants['f16_groupnorm_' + ('on_load' if args.separate_groupnorm else 'separate_pass')] = dict(
-            value=round(B / (N_SAMPLER_STEPS * ms3 * 1e-3), 4), unit='images/s', ms_per_step=round(ms3, 4))
-        del plan3, model3
         # A/B of programmatic dependent launch (the headline plan uses the package default)
         torch.manual_seed(0)
-        model4 = NCSNpp(cfg, precision='f16', separate_groupnorm=args.separate_groupnorm, pdl=not model.pdl).to(dev)
+        model4 = NCSNpp(cfg, precision='f16', pdl=not model.pdl).to(dev)
         plan4 = native.match_pc_plan(sde=sde, model=model4, predictor=sampling.ReverseDiffusionPredictor,
                                      corrector=sampling.LangevinCorrector, shape=shape, snr=cfg.sampling.snr, n_steps=1,
                                      probability_flow=False, continuous=True, eps=1e-5, device=dev)
@@ -577,21 +574,19 @@ def run_gpu_arm(args):
         variants['f16_pdl_' + ('off' if model.pdl else 'on')] = dict(value=round(B / (N_SAMPLER_STEPS * ms4 * 1e-3), 4), unit='images/s',
                                                                    ms_per_step=round(ms4, 4))
         del plan4, model4
-        # A/B of the halo form of the 3x3 mainloop (headline: package default = swapped AND CTA-pair kernels) against one shifted
-        # tile load per filter tap (swapped kernel: in the halo form's chunk-major K order, bit-identical results - round 1's
-        # tap-major loop was ~5 % faster than this on those launches, profiles/r02_h1_*; pair kernel: round 1's tap-major
-        # loop), and against the halo form in the swapped kernel only
-        for hv, key in ((False, 'f16_halo_off_same_k_order'), (True, 'f16_halo_swapped_kernel_only')):
+        # A/B of the halo form of the 3x3 mainloop in the swapped kernel against one shifted tile load per filter tap
+        # (in the halo form's chunk-major K order: bit-identical results)
+        for hv, key in ((False, 'f16_halo_off_same_k_order'),):
           torch.manual_seed(0)
-          model5 = NCSNpp(cfg, precision='f16', separate_groupnorm=args.separate_groupnorm, halo=hv).to(dev)
+          model5 = NCSNpp(cfg, precision='f16', halo=hv).to(dev)
           plan5 = native.match_pc_plan(sde=sde, model=model5, predictor=sampling.ReverseDiffusionPredictor,
                                        corrector=sampling.LangevinCorrector, shape=shape, snr=cfg.sampling.snr, n_steps=1,
                                        probability_flow=False, continuous=True, eps=1e-5, device=dev)
           ms5 = timed_steps(plan5, x_host.to(dev), args.warmup, args.steps)
           variants[key] = dict(value=round(B / (N_SAMPLER_STEPS * ms5 * 1e-3), 4), unit='images/s', ms_per_step=round(ms5, 4))
           del plan5, model5
-    # ---- strong-scaling probe (SURVEY 8e): the same 1024-image job cut over 8 GPUs is 128 images per GPU; time that
-    # per-GPU share here and name the launches that under-fill the 148 SMs ----
+    # ---- strong-scaling probe: the same 1024-image job cut over 8 GPUs is 128 images per GPU; time that
+    # per-GPU share here and name the launches that under-fill the SMs ----
     strong = None
     if world == 1 and not args.no_strong and B == 1024:
       sb = 128
@@ -626,11 +621,10 @@ def run_gpu_arm(args):
                             batch_per_gpu=B, global_batch=B * world, sampler_steps=N_SAMPLER_STEPS,
                             step='one PC iteration = Langevin corrector + reverse-diffusion predictor (2 score evaluations)',
                             parallelism=f'{world} independent chains shards (weights broadcast once, no in-loop collective)',
-                            l2='per-step working set (activations) exceeds the 126 MB L2 by >100x; no explicit flush',
+                            l2='per-step working set (activations) exceeds the 50 MB L2 by >100x; no explicit flush',
                             weights='random init, init_scale=1, torch.manual_seed(0)', precision=args.precision,
-                            groupnorm='separate streaming pass' if args.separate_groupnorm else
-                            'applied on load by the consuming convolution where supported (256-channel outputs at 16x16 / 32x32), separate pass elsewhere',
-                            conv3x3_mainloop={True: 'halo form (three W-shifted halo copies per channel chunk) in the swapped kernel, one shifted tile per tap in CTA pairs', False: 'one shifted tile load per filter tap', 'pairs': 'halo form in swapped and CTA-pair kernels'}[model.halo]),
+                            conv3x3_mainloop='halo form (three W-shifted halo copies per channel chunk) in the swapped kernel, one shifted tile per tap elsewhere'
+                            if model.halo else 'one shifted tile load per filter tap'),
                 clocks=clk,
                 e2e=dict(value=round(e2e_value, 4), unit='images/s', h2d_bytes_per_step=int(np.prod(shape)) * 4,
                          d2h_bytes_per_step=int(np.prod(shape)) * 4, ms_per_step=round(ms_e2e / e2e_steps, 4)),
@@ -649,7 +643,7 @@ def run_gpu_arm(args):
     dist.destroy_process_group()
 
 
-# ---- secondary workloads (SURVEY 8 f2 / f3: the other reference configurations the engine runs) ---------------------------
+# ---- secondary workloads (the other reference configurations the engine runs) ---------------------------------------------
 # `python bench.py --workload NAME` prints ONE JSON line for a non-headline configuration on one GPU: same timing rules
 # (device-resident state, CUDA events, >= 3 warm-up steps), no CPU / reference / scaling legs.  Parity for these
 # configurations is held by tests/test_gpu_{ddpmpp,progressive,ode}.py; the headline line is unaffected.
@@ -667,11 +661,11 @@ def run_secondary_workload(args):
                             desc='NCSN++ cont. CelebA-HQ 256x256 VE-SDE PC sampler (configs/ve/celebahq_256_ncsnpp_continuous.py), 2000 steps'),
     'ffhq_1024_ve': dict(cfg=configs.ve_ffhq_1024_ncsnpp_continuous, sde=lambda: sde_lib.VESDE(0.01, 1348, 2000), batch=2, precision='tf32',
                          pred=sampling.ReverseDiffusionPredictor, corr=sampling.LangevinCorrector, eps=1e-5, snr=0.15, evals=2,
-                         desc='NCSN++ FFHQ 1024x1024 VE-SDE PC sampler (configs/ve/ffhq_ncsnpp_continuous.py; BASELINE configs[4] per-GPU share), 2000 steps'),
+                         desc='NCSN++ FFHQ 1024x1024 VE-SDE PC sampler (configs/ve/ffhq_ncsnpp_continuous.py), 2000 steps'),
     'celebahq_256_ddpmpp_subvp_ode': dict(cfg=configs.subvp_celebahq_256_ddpmpp_continuous, sde=lambda: sde_lib.subVPSDE(0.1, 20., 1000), batch=8, precision='f16',
                                           ode=True, eps=1e-3,
                                           desc='DDPM++ cont. CelebA-HQ 256 sub-VP probability-flow ODE sampler, RK45 rtol=atol=1e-5, state on the device '
-                                               '(BASELINE configs[3] per-GPU share)'),
+                                               '(per-GPU share of a batch-64 job on 8 GPUs)'),
   }[args.workload]
   cfg = W['cfg']()
   cfg.model.init_scale = 1.0
@@ -726,16 +720,15 @@ def main():
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--warmup', type=int, default=3)
   ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
-  ap.add_argument('--batch', type=int, default=1024, help='images per GPU (BASELINE.json configs[1]: 1024)')
+  ap.add_argument('--batch', type=int, default=1024, help='images per GPU (default 1024)')
   ap.add_argument('--cpu-batch', type=int, default=8, help='batch of the bounded CPU sample')
   ap.add_argument('--precision', default='f16', choices=['tf32', 'f16', 'fp32'],
                   help="tensor-core operand format: 'f16' (default) and 'tf32' both carry 11-bit significands with fp32 "
                        "accumulation and meet the same 1e-3 parity bound (tests/test_gpu_tc.py); 'fp32' = CUDA cores")
   ap.add_argument('--no-variants', action='store_true', help='skip timing the other operand format')
-  ap.add_argument('--separate-groupnorm', dest='separate_groupnorm', action='store_true', default=SEPARATE_GROUPNORM_DEFAULT,
-                  help='GroupNorm+SiLU as stand-alone streaming passes (round-1 plan)')
-  ap.add_argument('--groupnorm-on-load', dest='separate_groupnorm', action='store_false',
-                  help='GroupNorm+SiLU applied on load by the consuming convolution where supported (csrc/gemm_tcg.cuh)')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='after the timed steps, write the last step\'s outputs (x.npy, x_mean.npy, float32, at most 64 MB: a fixed '
+                       'seeded subset of images above that; rank 0\'s shard under torch.distributed) to DIR')
   ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
   ap.add_argument('--no-strong', action='store_true', help='skip the 128-images-per-GPU strong-scaling probe')
   ap.add_argument('--parity-steps', type=int, default=10,

@@ -1,4 +1,4 @@
-/* scoresde_b200 — C ABI of the B200 (sm_100a) score-SDE sampling engine.
+/* scoresde_b200 — C ABI of the score-SDE sampling engine (sm_90a, H100).
  *
  * Drop-in boundary for the native surface of yang-song/score_sde_pytorch on the
  * predictor–corrector sampling path.  Every entry point takes plain pointers and
@@ -61,22 +61,22 @@ B200_API int b200_randn_like_torch_f32(float* out, long long numel, unsigned lon
                                        unsigned long long* offset_ws_dev /* 8 B device scratch */, void* stream);
 
 /* ---- one contraction (3x3 / 1x1 convolution on NHWC, 'same' padding, stride 1) ----
- * Exported so the tcgen05 path can be checked against the CUDA-core path and torch.
+ * Exported so the tensor-core path can be checked against the CUDA-core path and torch.
  * w_packed is [taps][c_out][c_in] (see b200_pack_conv_weight_f32). impl: 0 = fp32 CUDA cores,
- * 1 = tcgen05 TF32 (inputs must already be TF32-representable for exactness claims),
- * 2 = tcgen05 fp16: x1, x2 and w_packed hold IEEE fp16 elements (same layouts; round_tf32 = 2 packs / stores fp16);
+ * 1 = tensor-core TF32 (inputs must already be TF32-representable for exactness claims),
+ * 2 = tensor-core fp16: x1, x2 and w_packed hold IEEE fp16 elements (same layouts; round_tf32 = 2 packs / stores fp16);
  *     out is fp32 unless round_tf32 == 2;
  * 3 = warp-level TF32 MMAs for few-channel layers (c1, c2 multiples of 16, c_out 16 / 32 / 64, h % 8 == 0, w % 32 == 0):
  *     fp32 in and out, operands rounded to the TF32 grid while staged (the 16..64-channel levels of the nf = 16
  *     high-resolution networks, configs/ve/ffhq_ncsnpp_continuous.py:71-94);
- * 4 / 5 = as 1 / 2 with the halo form of the 3x3 mainloop disabled (nine shifted tile loads per channel chunk), 6 / 7 = as 1 / 2
- *     with the halo form in the CTA-pair kernel as well (b200_ncsnpp_config.no_halo = 1 / 2): A/B checks, bit-identical results. */
+ * 4 / 5 = as 1 / 2 with the halo form of the 3x3 mainloop disabled (nine shifted tile loads per channel chunk;
+ *     b200_ncsnpp_config.no_halo = 1): A/B checks, bit-identical results. */
 B200_API int b200_conv_nhwc_f32(const float* x1, int c1, const float* x2, int c2, int batch, int h, int w,
                                 const float* w_packed, const float* bias, int c_out, int ksize,
                                 const float* rowvec, long long rowvec_ld, const float* residual, float scale,
                                 int round_tf32, float* out, int impl, void* stream);
 /* 3x3 convolution with a fused 1x1 skip projection (a BigGAN resblock's tail, layerspp.py:268-274):
- * out = (conv3x3(x; w) + bias + [s1 | s2] w_skip^T + bias_skip + residual) * scale, tcgen05 path only.
+ * out = (conv3x3(x; w) + bias + [s1 | s2] w_skip^T + bias_skip + residual) * scale, tensor-core path only.
  * w_skip is [c_out][cs1 + cs2]; s1/s2 are NHWC tensors of the output's spatial size. */
 B200_API int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int cs1, const float* s2, int cs2,
                                      int batch, int h, int w, const float* w_packed, const float* bias,
@@ -85,7 +85,7 @@ B200_API int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int
 B200_API int b200_pack_conv_weight_f32(const float* w_oihw, float* w_packed, int c_out, int c_in, int ksize,
                                        int round_tf32, void* stream);
 /* Fused attention core of AttnBlockpp (layerspp.py:82-91) for T=256 tokens x C=256 channels per image:
- * out = (softmax(q k^T / sqrt(C)) v + b_v) W3^T + b_3 + x) * out_scale, tcgen05 only.
+ * out = (softmax(q k^T / sqrt(C)) v + b_v) W3^T + b_3 + x) * out_scale, tensor cores only.
  * qk = [nimg*T][2C] (q | k), vT = [nimg][C][T] (v transposed, without b_v), w3 = [C_out][C_in]; TF32-representable
  * fp32 (operand_f16 = 0) or IEEE fp16 elements (operand_f16 = 1).
  * qstats (optional, zero-initialised by the caller) receives out's GroupNorm quad sums [nimg][C/4][2]. */
@@ -117,15 +117,13 @@ typedef struct {
                                  * fp32 accumulation; activations between layers stay fp32) */
   int keep_activations;         /* debug: never recycle activation buffers so b200_ncsnpp_tap works */
   int lanes;                    /* 0/1: one plan over the whole batch (default); 2: two half-batch plans on two
-                                 * streams (batches >= 128).  Measured: no gain on a power-capped B200, see DESIGN.md */
+                                 * streams (batches >= 128).  Off by default. */
   int cuda_core_head;           /* 1: the output convolution (ncsnpp.py:374-380) runs on CUDA cores with an fp32 input in
                                  * every precision mode (costs ~1.4 % of a step, buys back ~1e-4 of rel-L2); 0: tensor cores */
-  int separate_groupnorm;       /* 1: every GroupNorm+SiLU as its own streaming pass (the round-1 plan, kept for A/B and
-                                 * as the checked alternative); 0: in fp16 operand mode GroupNorm+SiLU is applied ON LOAD by
-                                 * the consuming 3x3 convolution (csrc/gemm_tcg.cuh) wherever the shape allows
-                                 * (256-channel outputs at 16x16 / 32x32), so the normalised tensor never reaches HBM.
-                                 * The few-channel convolutions of the nf = 16 networks (csrc/conv_lowc.cu, TF32 mode) are
-                                 * memory-bound and apply their GroupNorm+SiLU on load under 0 and 1; 2: separate passes there too */
+  int separate_groupnorm;       /* 1: every GroupNorm+SiLU of the tensor-core layers is its own streaming pass; the few-channel
+                                 * convolutions of the nf = 16 networks (csrc/conv_lowc.cu, TF32 mode) are memory-bound and apply
+                                 * their GroupNorm+SiLU on load; 2: separate passes there too.  0 (GroupNorm on load by the
+                                 * tensor-core convolution) is not available in this build and is rejected by b200_ncsnpp_create. */
   int embedding_type;           /* 0: Gaussian Fourier features of log(sigma) (layerspp.py:32-41, all_modules[0].W); 1: sinusoidal
                                  * positional embedding of the time label (layers.py:515-529, ncsnpp.py:242-247): no module,
                                  * the frequency table is the pseudo-parameter "pos_freqs" [nf/2] */
@@ -136,15 +134,14 @@ typedef struct {
                                  * (the high-resolution NCSN++ family: configs/ve/{ffhq,celebahq}_*_ncsnpp_continuous.py) */
   int pdl;                      /* 1: every launch of a forward / PC iteration carries the programmatic-dependent-launch attribute
                                  * (each kernel waits for its predecessor with griddepcontrol.wait after its own prologue, so launch
-                                 * latency, barrier init and TMEM allocation of kernel k+1 overlap the tail of kernel k) */
-  int no_halo;                  /* (the Python host sets 2 unless told otherwise.)  0: swapped-form 3x3 convolutions (128 output channels) on 16- / 32-pixel-wide images read
-                                 * three W-shifted halo copies of their tile per channel chunk (csrc/gemm_tc.cu "halo form": 2.4x fewer
-                                 * L2 -> shared-memory bytes than one shifted tile per filter tap; measured +5..10 % on those launches);
-                                 * 1: one shifted tile per tap everywhere (the round-1 mainloop, kept for A/B); 2: halo form in the
-                                 * CTA-pair kernel as well (DESIGN.md section 4.13); + 4: with an L2 prefetch of the next tile's halo
-                                 * boxes (measured 2 % slower); + 8: small launches that fall back to the single-CTA kernel walk K in the halo form's
-                                 * order, so a small-batch plan agrees bit for bit with the pair plan of a large batch (tests).  Swapped-form results are bit-identical in every mode (same products, same order); the
-                                 * pair kernel's halo form walks K chunk-major, its nine-load form tap-major: fp32 summation order differs. */
+                                 * latency and barrier init of kernel k+1 overlap the tail of kernel k) */
+  int no_halo;                  /* (the Python host sets 2 unless told otherwise.)  0 or 2: swapped-form 3x3 convolutions (128 output channels) on
+                                 * 16- / 32-pixel-wide images read three W-shifted halo copies of their tile per channel chunk (csrc/gemm_tc.cu
+                                 * "halo form": 2.4x fewer L2 -> shared-memory bytes than one shifted tile per filter tap); 1: one shifted
+                                 * tile per tap everywhere (kept for A/B); + 4: with an L2 prefetch of the next tile's halo boxes; + 8:
+                                 * row-major launches of shapes with a halo form walk K in that form's order, so plans of different batch
+                                 * sizes agree bit for bit (tests).  Swapped-form results are bit-identical in every mode (same products,
+                                 * same order). */
 } b200_ncsnpp_config;
 
 B200_API int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out);
@@ -167,7 +164,7 @@ B200_API int b200_ncsnpp_forward(b200_ncsnpp_t* h, const float* x_nchw, const fl
 B200_API int b200_ncsnpp_tap(b200_ncsnpp_t* h, int module_index, float* dst_nchw, long long dst_cap_elems,
                              int shape_out[4], void* stream);
 B200_API long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h);
-/* One eager forward with a CUDA-event pair around every op; per-kind totals (kind 0 tcgen05
+/* One eager forward with a CUDA-event pair around every op; per-kind totals (kind 0 tensor-core
  * contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc):
  * device milliseconds, algorithmic FLOPs (2*M*N*K of the contractions) and op counts. */
 B200_API int b200_ncsnpp_profile_forward(b200_ncsnpp_t* h, const float* x_nchw, const float* labels,

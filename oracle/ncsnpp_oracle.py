@@ -10,7 +10,7 @@ Pinning: ``tools/make_golden.py`` runs the *real* reference
 inputs with weights loaded from the same ``state_dict`` and commits small
 fixtures under ``tests/golden/``; ``tests/test_oracle_golden.py`` checks this
 file against them.  The ``state_dict`` key names are the reference's
-(``all_modules.{i}.…``, SURVEY.md Appendix D-3), so a reference checkpoint loads
+(``all_modules.{i}.…``), so a reference checkpoint loads
 unchanged.
 
 Each function cites the reference lines it follows.  The arithmetic is written

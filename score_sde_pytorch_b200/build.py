@@ -1,4 +1,4 @@
-"""In-tree nvcc build of the C-ABI library ``libscoresde_b200.so`` for sm_100a.
+"""In-tree nvcc build of the C-ABI library ``libscoresde_b200.so`` for sm_90a.
 
 No torch headers are involved: the library is plain CUDA C++ behind ``extern "C"``
 entry points (``include/scoresde_b200.h``) and is loaded with ``ctypes``.  The
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libscoresde_b200.so')
 STAMP = os.path.join(HERE, '.libscoresde_b200.stamp')
 SOURCES = ['api.cu', 'elementwise.cu', 'conv_simt.cu', 'conv_lowc.cu', 'gemm_tc.cu', 'pc_update.cu', 'engine.cu', 'ode.cu', 'losses.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC,-fvisibility=hidden', '--expt-relaxed-constexpr']
 
 
@@ -40,7 +40,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-  """Compile every CUDA translation unit for sm_100a and link the shared library.
+  """Compile every CUDA translation unit for sm_90a and link the shared library.
   Returns the library path.  Skips the work when sources are unchanged."""
   digest = _digest()
   if not force and os.path.exists(LIB) and os.path.exists(STAMP):
@@ -63,7 +63,7 @@ def build(force=False, verbose=False):
     if verbose:
       print(out)
     objs.append(obj)
-  cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+  cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs
   r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
   if r.returncode != 0:
     raise RuntimeError(f'link failed:\n{r.stdout}')

@@ -196,8 +196,7 @@ def tiny_progressive(nf=32, image_size=32, num_res_blocks=1, ch_mult=(1, 1, 2), 
 
 
 def subvp_celebahq_256_ddpmpp_continuous():
-  """BASELINE.json configs[3]: "DDPM++ cont. CelebA-HQ 256 sub-VP".  The reference ships no such config file; as SURVEY
-  section 8(f) notes it is composed from ``configs/subvp/cifar10_ddpmpp_continuous.py`` (DDPM++: ``fir=False``, positional
+  """DDPM++ cont. CelebA-HQ 256 sub-VP.  The reference ships no such config file; it is composed from ``configs/subvp/cifar10_ddpmpp_continuous.py`` (DDPM++: ``fir=False``, positional
   embedding, no pyramids, sub-VP SDE, Euler-Maruyama predictor) with the 256-pixel data / ``ch_mult`` fields of
   ``configs/ve/celebahq_256_ncsnpp_continuous.py``."""
   c = subvp_cifar10_ddpmpp_continuous()

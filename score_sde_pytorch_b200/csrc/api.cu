@@ -103,9 +103,9 @@ int b200_conv_nhwc_f32(const float* x1, int c1, const float* x2, int c2, int bat
   ep.bias = bias; ep.rowvec = rowvec; ep.rowvec_ld = rowvec_ld; ep.residual = residual; ep.ld_res = c_out;
   ep.scale = scale; ep.round_tf32 = round_tf32; ep.rows_per_img = h * w; ep.out = out; ep.ld_out = c_out;
   if (!x2) c2 = 0;
-  if (impl == 1 || impl == 2 || (impl >= 4 && impl <= 7)) {   // 4 / 5: as 1 / 2 without the halo form; 6 / 7: halo form in CTA pairs too
+  if (impl == 1 || impl == 2 || impl == 4 || impl == 5) {   // 4 / 5: as 1 / 2 without the halo form
     TcGemmDesc d; memset(&d, 0, sizeof(d));
-    d.f16 = impl == 2 || impl == 5 || impl == 7; d.no_halo = impl >= 6 ? 2 : impl >= 4 ? 1 : 0;
+    d.f16 = impl == 2 || impl == 5; d.no_halo = impl >= 4 ? 1 : 0;
     d.a1 = x1; d.C1 = c1; d.a2 = x2; d.C2 = c2; d.conv = 1; d.H = h; d.W = w; d.nimg = batch; d.taps = ksize * ksize;
     d.w = w_packed; d.N_total = c_out; d.K_total = c1 + c2; d.w_rows = (long long)ksize * ksize * c_out; d.nbatch = 1;
     d.epi = ep;

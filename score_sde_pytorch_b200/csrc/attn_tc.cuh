@@ -2,27 +2,22 @@
 // C = 256 channels per image: logits, softmax, P.V, the output projection NIN_3, the residual add, the 1/sqrt(2)
 // rescale and the next GroupNorm's quad sums in ONE kernel, so the [T,T] logits / probabilities and the
 // attention output never touch HBM.  Included by gemm_tc.cu inside its anonymous namespace (PTX wrappers,
-// descriptors, quad_stats helper).
+// descriptors, fragment epilogue).
 //
 // One tile = 128 query rows of one image (two tiles per image); persistent CTAs, 384 threads:
-//   warp 0 lane 0  TMA producer: 24 loads per tile through a 2-stage ring of 48 KB slots
+//   warp 0         TMA producer (one elected lane issues): 24 loads per tile through a ring of 48 KB slots
 //                  (8 x {Q 128x32 + K 256x32}, 8 x V^T 256x32 keys, 8 x W3 256x32), running ahead across phases;
-//   warp 1 lane 0  MMA issuer, three chained contractions per tile, all M=128 x N=256 x K=256 (tf32):
-//                    S = Q K^T           -> TMEM columns [0,256)
-//                    O = E V             -> TMEM columns [256,512)   (A operand = E from shared memory)
-//                    Y = O' W3^T         -> TMEM columns [256,512)   (A operand = O' from shared memory)
-//   warp 2         TMEM allocation (all 512 columns);
-//   warps 4..11    two warps per TMEM lane quarter, each owning 128 of the 256 columns of its rows:
-//                    softmax : row max (exchange with the partner warp), E = exp((s-max)/sqrt(C)) rounded to TF32
-//                              into the 128 KB K-major SWIZZLE_128B operand buffer, row sums kept in registers;
-//                    convert : O' = O / rowsum + b_v (softmax rows sum to 1, so V's bias is added after P.V),
-//                              rounded to TF32 into the same operand buffer (E is dead once O is complete);
-//                    final   : (Y + b_3 + x) / sqrt(2), GroupNorm quad sums, direct 128-bit stores.
-// The issuer starts the next tile's S while the epilogue warps are still in `final` (S columns are free since
-// the softmax), so only the softmax and convert phases expose tensor-pipe bubbles.
+//   warps 4..11    two MMA warpgroups, warpgroup g owning query rows 64g .. 64g + 63 of the tile, three chained
+//                  m64 x n256 x k256 wgmma contractions with the accumulator in registers:
+//                    S = Q K^T    then softmax in registers (a row lives in one quad of lanes): E = exp((s-max)/sqrt(C))
+//                                 rounded to the operand format into the K-major SWIZZLE_128B operand buffer;
+//                    O = E V      (A operand = E from shared memory), then O' = O / rowsum + b_v (softmax rows sum to 1,
+//                                 so V's bias is added after P.V) rounded into the same buffer;
+//                    Y = O' W3^T  (A operand = O'), then (Y + b_3 + x) / sqrt(2), GroupNorm quad sums, direct stores.
+// A warpgroup only reads and writes its own 64 rows of the operand buffer, so it synchronises with itself alone.
 //
-// Deferred normalisation: the reference rounds nothing; here E (not E/rowsum) is the TF32 operand and the
-// division happens in fp32 on the accumulator - one rounding per operand, as everywhere else in the engine.
+// Deferred normalisation: the reference rounds nothing; here E (not E/rowsum) is the operand and the division
+// happens in fp32 on the accumulator - one rounding per operand, as everywhere else in the engine.
 
 // Operand formats: TF32-grid fp32 (kind::tf32; a 128-byte K block = 32 elements, 8 K blocks per contraction,
 // 128 KB operand buffer, 2-stage ring) or fp16 (kind::f16; 64 elements per K block, 4 K blocks, 64 KB operand
@@ -36,10 +31,9 @@ struct AttnSmem {
   static constexpr int RING = KB * 16384;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + 256 * 128;     // 16 KB + 32 KB
   static constexpr int STAGES = F16 ? 3 : 2;
-  static constexpr int XCHG = RING + STAGES * STAGE_BYTES;          // [2 halves][128 rows] floats
-  static constexpr int BAR_OFFSET = XCHG + 1024;
+  static constexpr int BAR_OFFSET = RING + STAGES * STAGE_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB shared-memory limit of sm_100");
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB shared-memory limit of sm_90");
 };
 
 struct AttnParams {
@@ -58,29 +52,38 @@ struct AttnParams {
 __device__ __forceinline__ uint8_t* pbuf_chunk(uint8_t* pbuf, int kb, int r, int c16) {
   return pbuf + kb * 16384 + (r >> 3) * 1024 + (r & 7) * 128 + ((c16 ^ (r & 7)) << 4);
 }
-// write 32 consecutive K elements (k0 .. k0+31, k0 % 32 == 0) of operand row r: TF32-rounded fp32 or fp16
+// write K elements k, k + 1 (k even) of operand row r: TF32-rounded fp32 or fp16
 template <bool F16>
-__device__ __forceinline__ void pbuf_store32(uint8_t* pbuf, int r, int k0, const float (&v)[32]) {
+__device__ __forceinline__ void pbuf_store2(uint8_t* pbuf, int r, int k, float a, float b) {
   if (F16) {
-    const int kb = k0 >> 6, c0 = (k0 & 63) >> 3;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      uint4 u;
-      u.x = pack_half2(v[8 * c], v[8 * c + 1]); u.y = pack_half2(v[8 * c + 2], v[8 * c + 3]);
-      u.z = pack_half2(v[8 * c + 4], v[8 * c + 5]); u.w = pack_half2(v[8 * c + 6], v[8 * c + 7]);
-      sts128(smem_u32(pbuf_chunk(pbuf, kb, r, c0 + c)), u.x, u.y, u.z, u.w);
-    }
+    const uint32_t sa = smem_u32(pbuf_chunk(pbuf, k >> 6, r, (k & 63) >> 3)) + (k & 7) * 2;
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(sa), "r"(pack_half2(a, b)) : "memory");
   } else {
-    const int kb = k0 >> 5;
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-      sts128(smem_u32(pbuf_chunk(pbuf, kb, r, c)), __float_as_uint(round_tf32(v[4 * c])), __float_as_uint(round_tf32(v[4 * c + 1])),
-             __float_as_uint(round_tf32(v[4 * c + 2])), __float_as_uint(round_tf32(v[4 * c + 3])));
+    const uint32_t sa = smem_u32(pbuf_chunk(pbuf, k >> 5, r, (k & 31) >> 2)) + (k & 3) * 4;
+    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(sa), "r"(__float_as_uint(round_tf32(a))), "r"(__float_as_uint(round_tf32(b))) : "memory");
   }
 }
-__device__ __forceinline__ float lds32(uint32_t saddr) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr)); return v; }
-__device__ __forceinline__ void sts32(uint32_t saddr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory"); }
-__device__ __forceinline__ void pair_barrier(int q) { asm volatile("bar.sync %0, 64;" ::"r"(q + 1) : "memory"); }
+
+// One contraction of the tile: KB ring slots, B operand from the slot, A from the slot (phase 0) or the operand buffer.
+template <bool F16>
+__device__ __forceinline__ void attn_phase(float (&acc)[128], int ph, uint8_t* ring, uint8_t* pbuf, uint64_t* full_bar,
+                                           uint64_t* empty_bar, uint32_t& stage, uint32_t& phase, int g, int lane) {
+  using L = AttnSmem<F16>;
+  int pend = -1;
+#pragma unroll 1
+  for (int kc = 0; kc < L::KB; ++kc) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_u32(ring + stage * L::STAGE_BYTES);
+    const uint32_t a = ph == 0 ? sa : smem_u32(pbuf + kc * 16384);
+    wgmma_kstep<256, F16>(acc, make_smem_desc(a + g * (A_STAGE_BYTES / 2)), make_smem_desc(sa + A_STAGE_BYTES), kc);
+    wgmma_wait<1>();
+    if (lane == 0 && pend >= 0) mbar_arrive(&empty_bar[pend]);
+    pend = (int)stage;
+    if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  if (lane == 0) mbar_arrive(&empty_bar[pend]);
+}
 
 template <bool F16>
 __global__ void __launch_bounds__(384, 1) attn_tc_kernel(const __grid_constant__ AttnParams p) {
@@ -89,42 +92,28 @@ __global__ void __launch_bounds__(384, 1) attn_tc_kernel(const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* pbuf = smem + L::PBUF;
   uint8_t* ring = smem + L::RING;
-  float* xchg = reinterpret_cast<float*>(smem + L::XCHG);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + L::STAGES;
-  uint64_t* s_full = empty_bar + L::STAGES;
-  uint64_t* p_ready = s_full + 1;
-  uint64_t* o_full = p_ready + 1;
-  uint64_t* o_ready = o_full + 1;
-  uint64_t* y_full = o_ready + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(y_full + 1);
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp index provably warp-uniform
   if (threadIdx.x == 0) {
-    for (int s = 0; s < L::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(s_full, 1); mbar_init(o_full, 1); mbar_init(y_full, 1);
-    mbar_init(p_ready, 8); mbar_init(o_ready, 8);
+    for (int s = 0; s < L::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // one arrival per MMA warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait(); pdl_trigger();   // prologue done; nothing above touched global memory (common.cuh)
   const long long total_tiles = 2LL * p.nimg;
   constexpr int KB = L::KB;        // K blocks in every phase (C = T = 256 elements)
   constexpr int BKA = L::BKA;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    regs_producer();
+    if (warp != 0) return;
     // ======================= TMA producer (whole warp; one elected lane issues - see elect_one in gemm_tc.cu) =======================
     const bool issue = elect_one();
     uint32_t stage = 0, phase = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int b = (int)(tile >> 1), qh = (int)(tile & 1);
       for (int ph = 0; ph < 3; ++ph) {
         for (int kc = 0; kc < KB; ++kc) {
@@ -147,133 +136,69 @@ __global__ void __launch_bounds__(384, 1) attn_tc_kernel(const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer (whole warp; one elected lane issues) =======================
-    const bool issue = elect_one();
-    constexpr uint32_t idesc = F16 ? make_idesc_f16<256>() : make_idesc<256>();
-    uint32_t stage = 0, phase = 0, tpar = 0;
-    const uint32_t s_tmem = tmem_base, o_tmem = tmem_base + 256;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tpar ^= 1) {
-      for (int ph = 0; ph < 3; ++ph) {
-        if (ph == 1) { mbar_wait(p_ready, tpar); tc_fence_after(); }   // E is in shared memory
-        if (ph == 2) { mbar_wait(o_ready, tpar); tc_fence_after(); }   // O' is in shared memory, O columns drained
-        const uint32_t d_tmem = ph == 0 ? s_tmem : o_tmem;
-        for (int kc = 0; kc < KB; ++kc) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(ring + stage * L::STAGE_BYTES);
-          const uint64_t adesc = make_smem_desc(ph == 0 ? sa : smem_u32(pbuf + kc * 16384));
-          const uint64_t bdesc = make_smem_desc(sa + A_STAGE_BYTES);
-          if (issue) {
-            umma_kstep<F16>(d_tmem, adesc, bdesc, idesc, kc);
-            umma_commit(&empty_bar[stage]);
-          }
-          if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (issue) umma_commit(ph == 0 ? s_full : ph == 1 ? o_full : y_full);
-      }
-    }
-  } else if (warp >= 4) {
-    // ======================= softmax / convert / final =======================
-    const int q = (warp - 4) & 3, half = (warp - 4) >> 2;
-    const int r = q * 32 + lane;                       // query row of the tile == TMEM lane
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t tpar = 0;
-    for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tpar ^= 1) {
-      const int b = (int)(tile >> 1), qh = (int)(tile & 1);
-      const long long gm = (long long)b * AT_T + qh * BM + r;
-#pragma unroll
-      for (int i = 0; i < 128; i += 32) prefetch_l2(p.x + gm * AT_C + half * 128 + i);   // residual row -> L2 for `final`
-      // ---- softmax over this row's 256 logits (this thread: columns half*128 .. +128) ----
-      mbar_wait(s_full, tpar);
-      tc_fence_after();
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        uint32_t v[32];
-        tmem_ld32(lane_addr + half * 128 + j * 32, v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-      }
-      const uint32_t xmine = smem_u32(xchg) + (half * 128 + r) * 4, xother = smem_u32(xchg) + ((half ^ 1) * 128 + r) * 4;
-      sts32(xmine, mx);
-      pair_barrier(q);
-      mx = fmaxf(mx, lds32(xother));
-      const float moff = mx * p.logit_scale;
-      float sum = 0.f;
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        uint32_t v[32];
-        tmem_ld32(lane_addr + half * 128 + j * 32, v);
-        float ev[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          ev[c] = exp2f(fmaf(__uint_as_float(v[c]), p.logit_scale, -moff));
-          sum += ev[c];
-        }
-        pbuf_store32<F16>(pbuf, r, half * 128 + j * 32, ev);
-      }
-      pair_barrier(q);                                  // the partner has read this thread's max: the slot is free
-      sts32(xmine, sum);
-      fence_async_smem();                               // E (generic-proxy writes) -> visible to the tensor core
-      pair_barrier(q);
-      sum += lds32(xother);
-      const float inv = 1.0f / sum;
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-      // ---- O' = O / rowsum + b_v -> operand buffer (K = channel) ----
-      mbar_wait(o_full, tpar);
-      tc_fence_after();
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {
-        uint32_t v[32];
-        tmem_ld32(lane_addr + 256 + half * 128 + j * 32, v);
-        const int ch0 = half * 128 + j * 32;
-        const float* bvp = p.bv + ch0;
-        float ov[32];
-#pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          const float4 t = __ldg(reinterpret_cast<const float4*>(bvp + c));
-          ov[c] = fmaf(__uint_as_float(v[c]), inv, t.x);
-          ov[c + 1] = fmaf(__uint_as_float(v[c + 1]), inv, t.y);
-          ov[c + 2] = fmaf(__uint_as_float(v[c + 2]), inv, t.z);
-          ov[c + 3] = fmaf(__uint_as_float(v[c + 3]), inv, t.w);
-        }
-        pbuf_store32<F16>(pbuf, r, ch0, ov);
-      }
-      fence_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_ready);
-      // ---- final: (Y + b_3 + x) * out_scale, quad sums, store ----
-      // Through the same coalescing block routine as the convolution epilogues.  Its 4 KB transposition scratch is
-      // this warp's slice of the operand buffer: O' is dead once Y is complete, and the slice (rows of this warp's
-      // lane quarter in K block `half`) is next written by the quarter's half-0 warp only after the pair barrier of
-      // the next tile's softmax, i.e. after this warp has left `final`.
-      mbar_wait(y_full, tpar);
-      tc_fence_after();
-      {
-        Epilogue ep;
-        ep.bias = p.b3; ep.rowvec = nullptr; ep.rowvec_ld = 0; ep.residual = p.x; ep.ld_res = AT_C; ep.per_img_div = nullptr;
-        ep.div_stride = 0; ep.scale = p.out_scale; ep.round_tf32 = 0; ep.rows_per_img = AT_T; ep.out = p.out; ep.ld_out = AT_C;
-        ep.out_nchw = 0;
-        const long long gm0 = (long long)b * AT_T + qh * BM + q * 32;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          uint32_t v[32];
-          tmem_ld32(lane_addr + 256 + half * 128 + j * 32, v);
-          if (p.qstats) row_chunk_t<true, 0, true>(v, pbuf + (warp - 4) * 4096, ep, p.qstats, AT_C, gm0, 32, half * 128 + j * 32, b, lane);
-          else row_chunk_t<true, 0, false>(v, pbuf + (warp - 4) * 4096, ep, p.qstats, AT_C, gm0, 32, half * 128 + j * 32, b, lane);
-        }
-      }
-      tc_fence_before();   // orders these TMEM reads before the p_ready arrival that lets the next tile's E V overwrite O/Y
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
+  regs_consumer();
+  // ======================= MMA warpgroups: softmax / convert / final =======================
+  const int g = (warp >> 2) - 1, wq = warp & 3;
+  const int ra = g * 64 + wq * 16 + (lane >> 2), rb = ra + 8;   // the two query rows of the tile this thread holds
+  uint32_t stage = 0, phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int b = (int)(tile >> 1), qh = (int)(tile & 1);
+    float acc[128];
+    // ---- S = Q K^T, softmax over each row's 256 logits (a quad of lanes holds a row) ----
+    attn_phase<F16>(acc, 0, ring, pbuf, full_bar, empty_bar, stage, phase, g, lane);
+    float mxa = -INFINITY, mxb = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      mxa = fmaxf(mxa, fmaxf(acc[4 * j], acc[4 * j + 1]));
+      mxb = fmaxf(mxb, fmaxf(acc[4 * j + 2], acc[4 * j + 3]));
+    }
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, m));
+      mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, m));
+    }
+    const float moffa = mxa * p.logit_scale, moffb = mxb * p.logit_scale;
+    float suma = 0.f, sumb = 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int k = 8 * j + 2 * (lane & 3);
+      const float e0 = exp2f(fmaf(acc[4 * j], p.logit_scale, -moffa)), e1 = exp2f(fmaf(acc[4 * j + 1], p.logit_scale, -moffa));
+      const float e2 = exp2f(fmaf(acc[4 * j + 2], p.logit_scale, -moffb)), e3 = exp2f(fmaf(acc[4 * j + 3], p.logit_scale, -moffb));
+      suma += e0 + e1; sumb += e2 + e3;
+      pbuf_store2<F16>(pbuf, ra, k, e0, e1);
+      pbuf_store2<F16>(pbuf, rb, k, e2, e3);
+    }
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      suma += __shfl_xor_sync(0xffffffffu, suma, m);
+      sumb += __shfl_xor_sync(0xffffffffu, sumb, m);
+    }
+    const float inva = 1.0f / suma, invb = 1.0f / sumb;
+    fence_async_smem();                               // E (generic-proxy writes) -> visible to the tensor core
+    wg_barrier(g);
+    // ---- O = E V;  O' = O / rowsum + b_v -> operand buffer (K = channel) ----
+    attn_phase<F16>(acc, 1, ring, pbuf, full_bar, empty_bar, stage, phase, g, lane);
+    wg_barrier(g);                                    // every warp of the warpgroup is done reading E
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const int ch = 8 * j + 2 * (lane & 3);
+      const float2 t = __ldg(reinterpret_cast<const float2*>(p.bv + ch));
+      pbuf_store2<F16>(pbuf, ra, ch, fmaf(acc[4 * j], inva, t.x), fmaf(acc[4 * j + 1], inva, t.y));
+      pbuf_store2<F16>(pbuf, rb, ch, fmaf(acc[4 * j + 2], invb, t.x), fmaf(acc[4 * j + 3], invb, t.y));
+    }
+    fence_async_smem();
+    wg_barrier(g);
+    // ---- Y = O' W3^T;  final: (Y + b_3 + x) * out_scale, quad sums, store ----
+    attn_phase<F16>(acc, 2, ring, pbuf, full_bar, empty_bar, stage, phase, g, lane);
+    wg_barrier(g);                                    // O' is dead: the next tile's E may overwrite it
+    Epilogue ep;
+    ep.bias = p.b3; ep.rowvec = nullptr; ep.rowvec_ld = 0; ep.residual = p.x; ep.ld_res = AT_C; ep.per_img_div = nullptr;
+    ep.div_stride = 0; ep.scale = p.out_scale; ep.round_tf32 = 0; ep.rows_per_img = AT_T; ep.out = p.out; ep.ld_out = AT_C;
+    ep.out_nchw = 0; ep.n_valid = 0;
+    const long long gm = (long long)b * AT_T + qh * BM + g * 64 + wq * 16;
+    if (p.qstats) frag_rows<256, true, 0, true>(acc, ep, p.qstats, AT_C, gm, 16, 0, lane);
+    else frag_rows<256, true, 0, false>(acc, ep, p.qstats, AT_C, gm, 16, 0, lane);
   }
 }

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the score-SDE sampling engine.
+// Shared helpers for the sm_90a kernels of the score-SDE sampling engine.
 // Error reporting follows the C-ABI contract in include/scoresde_b200.h:
 // every entry point returns 0 on success, non-zero on failure, and the text is
 // available from b200_last_error().
@@ -42,7 +42,7 @@ static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) 
 // ---- device helpers --------------------------------------------------------
 __device__ __forceinline__ float round_tf32(float x) {
   // round-to-nearest (ties away) to the 10-bit-mantissa TF32 grid, kept as fp32 bits.
-  // tcgen05 kind::tf32 ignores the low 13 mantissa bits of its operands; pre-rounding
+  // wgmma .tf32 ignores the low 13 mantissa bits of its operands; pre-rounding
   // makes that truncation a no-op so the only error is one RN rounding per operand.
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -52,8 +52,8 @@ __device__ __forceinline__ float round_tf32(float x) {
 // Operand-grid stores.  Tensors that feed a tensor-core contraction are written by their producer in one of
 // three forms, selected by an integer `mode` that travels with the launch:
 //   0  fp32 as computed;
-//   1  fp32 rounded to the TF32 grid (operands of tcgen05 kind::tf32);
-//   2  IEEE fp16, round-to-nearest-even (operands of tcgen05 kind::f16).  Same 11-bit significand as TF32, half the
+//   1  fp32 rounded to the TF32 grid (operands of wgmma .tf32);
+//   2  IEEE fp16, round-to-nearest-even (operands of wgmma .f16).  Same 11-bit significand as TF32, half the
 //      bytes in HBM and shared memory; `base` then addresses __half elements and `idx` counts halves.
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   uint32_t r;
@@ -84,7 +84,7 @@ __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x));
 // rcp.approx (relative error ~1e-6, two orders below the rounding) instead of the IEEE exp/divide sequences,
 // which made this HBM-streaming kernel instruction-bound (~25 -> ~8 instructions per element).
 // (Written out as the two MUFU ops: __fdividef / __expf wrap them in range-scaling code, 9-10 instructions per element
-// instead of 5; the convolution that applies GroupNorm on load, gemm_tcg.cuh, uses the same function so both plans round alike.)
+// instead of 5.)
 __device__ __forceinline__ float silu_fast(float x) {
   float e, r;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
@@ -112,7 +112,7 @@ __device__ __forceinline__ float warp_max(float v) {
 // Every kernel of this library starts with griddepcontrol.wait - which returns once the preceding kernel of the stream has
 // completed and its memory is visible, i.e. ordinary stream order - followed by griddepcontrol.launch_dependents, which
 // lets the NEXT kernel's CTAs be scheduled as soon as all of this kernel's CTAs are running.  The tensor-core kernels put
-// the pair after their prologue (barrier init, TMEM allocation), so that prologue and the launch latency of kernel k+1
+// the pair after their prologue (barrier init), so that prologue and the launch latency of kernel k+1
 // overlap the tail of kernel k (464 launches per PC step).  Without the launch attribute both instructions are no-ops.
 // Host side: launch_kernel() adds cudaLaunchAttributeProgrammaticStreamSerialization when the calling engine asked for it
 // (b200_ncsnpp_config.pdl; a thread-local scope set by the forward / PC-loop entry points - nothing process-global).

@@ -2,7 +2,7 @@
 //
 // These are the 1024..128-pixel levels of the high-resolution family (nf = 16: 16, 32, 64 channels;
 // /root/reference/configs/ve/ffhq_ncsnpp_continuous.py:71-94).  Their output tiles are far too narrow for the
-// tcgen05 tiling (N = 128 / 256 columns, K steps of 32 TF32 elements) and they are memory-bound by construction:
+// wgmma tiling (N = 128 / 256 columns, K steps of 32 TF32 elements) and they are memory-bound by construction:
 // 16 -> 16 channels is 36 FLOP per byte.  What they need is enough contraction rate to stay at the HBM roofline,
 // which the strict-fp32 CUDA-core kernel (conv_simt.cu: 6 - 28 TFLOP/s on these shapes, 73 % of an FFHQ-1024
 // evaluation) does not have and warp-level TF32 MMAs do:
@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(LC_THREADS, 2) conv_lowc_kernel(const SimtConv
 
 int lc_num_sms() {
   static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
   return n;
 }
 

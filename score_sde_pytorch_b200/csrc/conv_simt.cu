@@ -1,10 +1,10 @@
 // Strict-fp32 CUDA-core implicit GEMM.  It serves three purposes:
-//   * the layers whose shape does not fit the tcgen05 tiling (3->128 input conv read
+//   * the layers whose shape does not fit the tensor-core tiling (3->128 input conv read
 //     straight from NCHW, 128->3 output conv written straight to NCHW with the 1/sigma
 //     scaling fused, FIR-padded stride-2 pyramid convs, 4x4-resolution attention);
 //   * an exact-fp32 execution mode of the whole network (precision="fp32") used to
 //     separate logic errors from TF32 rounding when checking parity with the oracle;
-//   * the reference point the tcgen05 path is validated against on the device.
+//   * the reference point the tensor-core path is validated against on the device.
 // K is walked flat over (tap, channel) so tiny channel counts (Cin=3) do not waste
 // the K tile; operands are staged k-major in shared memory and every thread keeps a
 // TM x TN register tile.
@@ -172,12 +172,12 @@ int launch_conv_simt(const SimtConv& p, cudaStream_t st) {
   if (p.N <= 8) {
     constexpr int BM = 256, BN = 8;
     const long long tiles = (long long)p.nbatch * ceil_div(rows_per_img, BM) * ceil_div(p.N, BN);
-    const int grid = (int)std::min<long long>(tiles, 148LL * 8);
+    const int grid = (int)std::min<long long>(tiles, 132LL * 8);
     launch_kernel(conv_simt_kernel<BM, BN, 1, 8>, dim3(grid), dim3(256), 0, st, p);
   } else {
     constexpr int BM = 64, BN = 64;
     const long long tiles = (long long)p.nbatch * ceil_div(rows_per_img, BM) * ceil_div(p.N, BN);
-    const int grid = (int)std::min<long long>(tiles, 148LL * 8);
+    const int grid = (int)std::min<long long>(tiles, 132LL * 8);
     launch_kernel(conv_simt_kernel<BM, BN, 4, 4>, dim3(grid), dim3(256), 0, st, p);
   }
   B200_CHECK_LAUNCH();

@@ -19,7 +19,7 @@ namespace b200 {
 // channels the pair (sum x, sum x^2).  Any GroupNorm group of this network (4/8/12/16 channels,
 // always quad aligned, possibly straddling the two sources of a U-Net channel concat,
 // ncsnpp.py:318) is a sum of 1-4 quads, so a tensor's quad sums serve every consumer.  They are
-// produced for free by the tcgen05 contraction's epilogue (gemm_tc.cu) for tensors it writes, or
+// produced for free by the tensor-core contraction's epilogue (gemm_tc.cu) for tensors it writes, or
 // by gn_quad_stats_kernel below for the rest; gn_apply_kernel turns them into mean / rstd once
 // per thread and streams the tensor exactly once (read + write, optional TF32-rounded raw copy).
 // ============================================================================
@@ -203,8 +203,7 @@ __global__ void __launch_bounds__(GN_THREADS) gn_apply_kernel(
 }
 
 // ---- lean streaming form -------------------------------------------------------------------------------
-// The generic kernel above turned out instruction-bound (ncu, profiles/r01_c26_ncu_gn_apply.md: 26 instructions
-// per element, issue slots 78 % busy, DRAM 41-67 %): per-element guards, 64-bit index multiplies, both SiLU paths
+// The generic kernel above is instruction-bound (about 26 instructions per element): per-element guards, 64-bit index multiplies, both SiLU paths
 // compiled into one loop, and an fp64 divide + square root per thread.  Here every launch property is a template
 // parameter, the per-quad scale / shift (rstd*gamma, beta - mean*rstd*gamma) are computed once per CTA into shared
 // memory (fp64 only for mean and variance; the reciprocal square root is taken in fp32), the main loop runs
@@ -302,7 +301,7 @@ int launch_gn_apply(const float* x1, int C1, const float* x2, int C2, const doub
                "gn_apply: C=%d (C1=%d) G=%d must give 4-aligned groups", C, C1, G);
   const int Q = C / 4;
   // Small CTAs (the smallest multiple of the quad count >= 128 threads: 128 or 192 here): finer-grained tail, and
-  // several fit in the registers a persistent tcgen05 CTA leaves free (112 regs x 384 threads = 43 K of 64 K).
+  // several fit in the registers a persistent tensor-core CTA leaves free.
   int threads = GN_THREADS;
   for (int t = 128; t <= GN_THREADS; t += 32) if (t % Q == 0) { threads = t; break; }
   B200_REQUIRE(!x1_f16 || (threads % Q == 0 && !raw), "gn_apply: fp16 input needs the quad-per-thread path (C=%d) and no raw copy", C);
@@ -310,7 +309,7 @@ int launch_gn_apply(const float* x1, int C1, const float* x2, int C2, const doub
   const long long per_img_units = (long long)HW * Q;
   const int work = 16;
   // (few, very large images - the 1024-pixel family at batch 2 - need more than 64 CTAs per image to fill the chip)
-  const long long max_splits = std::max<long long>(64, (148LL * 16 + B - 1) / B);
+  const long long max_splits = std::max<long long>(64, (132LL * 16 + B - 1) / B);
   int splits = (int)std::max<long long>(1, std::min<long long>(per_img_units / ((long long)threads * work), max_splits));
   splits = std::min(splits, HW);
   dim3 grid(splits, B);
@@ -407,7 +406,7 @@ int launch_gn_generic(const float* x1, int C1, const float* x2, int C2, const fl
   launch_kernel(gn_generic_finish_kernel, dim3((B * G + 127) / 128), dim3(128), 0, st, (const double*)part, B * G, S,
                 (double)HW * (C / G), eps, mr);
   const long long total = (long long)B * HW * C;
-  const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 32);
+  const int grid = (int)std::min<long long>((total + 255) / 256, 132LL * 32);
   launch_kernel(gn_generic_apply_kernel, dim3(grid), dim3(256), 0, st, x1, C1, x2, C2, (const float2*)mr, gamma, beta, B, HW, G, act, round_out, y, raw);
   B200_CHECK_LAUNCH();
   return 0;
@@ -415,8 +414,8 @@ int launch_gn_generic(const float* x1, int C1, const float* x2, int C2, const fl
 
 // GroupNorm folded into per-(image, channel) affine coefficients: scale = rstd * gamma, shift = beta - mean * scale,
 // from the same fp64 quad sums and with the same fp32 operations as gn_apply_stream_kernel (so a consumer that applies
-// fma(x, scale, shift) reproduces that kernel bit for bit).  Consumed by the convolutions that normalise their input on
-// load (gemm_tcg.cuh): the [B][C] tables are ~1e-3 of the activation bytes, the normalised tensor is never stored.
+// fma(x, scale, shift) reproduces that kernel bit for bit).  Consumed by the few-channel convolutions that normalise their
+// input on load (conv_lowc.cu): the [B][C] tables are ~1e-3 of the activation bytes, the normalised tensor is never stored.
 __global__ void __launch_bounds__(128) gn_coeff_kernel(const double* __restrict__ q1, int C1, const double* __restrict__ q2, int C2,
                                                        const float* __restrict__ gamma, const float* __restrict__ beta, int G,
                                                        float eps, double inv_n, float* __restrict__ scale, float* __restrict__ shift) {
@@ -702,7 +701,7 @@ int launch_upfirdn2d(const float* x, const float* kernel_host, float* y, int maj
     B200_CHECK_LAUNCH();
     return 0;
   }
-  const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 64);
+  const int grid = (int)std::min<long long>((total + 255) / 256, 132LL * 64);
   if (vec) launch_kernel(upfirdn2d_kernel<4>, dim3(grid), dim3(256), 0, st, x, y, p);
   else launch_kernel(upfirdn2d_kernel<1>, dim3(grid), dim3(256), 0, st, x, y, p);
   B200_CHECK_LAUNCH();
@@ -737,7 +736,7 @@ int launch_fused_bias_act(const float* x, const float* b, const float* ref, floa
   if (n == 0) return 0;
   B200_REQUIRE(act == 1 || act == 3, "fused_bias_act: act=%d unsupported (1 linear, 3 lrelu)", act);
   B200_REQUIRE(!b || (step_b > 0 && size_b > 0), "fused_bias_act: bad bias geometry");
-  const int grid = (int)std::min<long long>((n + 255) / 256, 148LL * 64);
+  const int grid = (int)std::min<long long>((n + 255) / 256, 132LL * 64);
   launch_kernel(fused_bias_act_kernel, dim3(grid), dim3(256), 0, st, x, b, ref, y, n, step_b, size_b, act, grad, alpha, scale);
   B200_CHECK_LAUNCH();
   return 0;
@@ -825,7 +824,7 @@ int launch_softmax_rows(const float* s, float* p, long long rows, int T, float s
   B200_REQUIRE(T > 0 && T <= 1024, "softmax_rows: T=%d out of range (1..1024)", T);
   const int wpb = 8;
   if (T == 256 && ((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(p)) & 15) == 0) {
-    const long long blocks = std::min<long long>((rows / 2 + wpb - 1) / wpb + 1, 148LL * 16);
+    const long long blocks = std::min<long long>((rows / 2 + wpb - 1) / wpb + 1, 132LL * 16);
     launch_kernel(softmax_rows256_kernel, dim3((unsigned)blocks), dim3(wpb * 32), 0, st, s, p, rows, scale, round_out);
     B200_CHECK_LAUNCH();
     return 0;
@@ -906,7 +905,7 @@ int launch_linear_rows(const float* x, long long ldx, const float* W, const floa
   const size_t smem = (size_t)LIN_RB * K * sizeof(float);
   if (smem > 48 * 1024)
     B200_CHECK_CUDA(cudaFuncSetAttribute(linear_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid(std::min(ceil_div(N, 8), 148 * 4), ceil_div(rows, LIN_RB));
+  dim3 grid(std::min(ceil_div(N, 8), 132 * 4), ceil_div(rows, LIN_RB));   // 4 CTAs per H100 SM
   launch_kernel(linear_rows_kernel, dim3(grid), dim3(256), smem, st, x, ldx, W, bias, rows, N, K, act_in, y, ldy);
   B200_CHECK_LAUNCH();
   return 0;
@@ -941,7 +940,7 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ src, float* __rest
 }
 int launch_nhwc_to_nchw(const float* src, float* dst, int B, int HW, int C, cudaStream_t st) {
   const long long total = (long long)B * HW * C;
-  launch_kernel(nhwc_to_nchw_kernel, dim3((int)std::min<long long>((total + 255) / 256, 148LL * 64)), dim3(256), 0, st, src, dst, B, HW, C);
+  launch_kernel(nhwc_to_nchw_kernel, dim3((int)std::min<long long>((total + 255) / 256, 132LL * 64)), dim3(256), 0, st, src, dst, B, HW, C);
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -967,7 +966,7 @@ int launch_pack_weight(const float* src, float* dst, int taps, int O, int I, lon
                        long long stp, int round_out, cudaStream_t st, long long dt, long long dO) {
   const long long total = (long long)taps * O * I;
   if (dt == 0) { dt = (long long)O * I; dO = I; }
-  launch_kernel(pack_weight_kernel, dim3((int)std::min<long long>((total + 255) / 256, 148LL * 16)), dim3(256), 0, st, 
+  launch_kernel(pack_weight_kernel, dim3((int)std::min<long long>((total + 255) / 256, 132LL * 16)), dim3(256), 0, st, 
       src, dst, taps, O, I, so, si, stp, round_out, dt, dO);
   B200_CHECK_LAUNCH();
   return 0;
@@ -976,7 +975,7 @@ int launch_pack_weight(const float* src, float* dst, int taps, int O, int I, lon
 // ============================================================================
 // Input convolution as one K=32 contraction: patches[b*HW + pix][tap*C + c] = x[b][c][pix + tap offset]
 // (zero outside the image, zero for k >= 9*C), TF32-rounded, from the NCHW network input.
-// 9*C <= 32 (C = 3 for images).  The 3->nf 3x3 conv (ncsnpp.py:268) then runs on tcgen05 as a
+// 9*C <= 32 (C = 3 for images).  The 3->nf 3x3 conv (ncsnpp.py:268) then runs on the tensor cores as a
 // [B*HW, 32] x [nf, 32]^T product instead of a 27-deep CUDA-core loop.
 // ============================================================================
 template <int C>   // image channels (9*C <= 32); compile-time so the patch lives in registers

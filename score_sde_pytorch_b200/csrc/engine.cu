@@ -14,7 +14,6 @@
 
 namespace b200 {
 void tc_gemm_set_rowvec_ld(TcGemmPlan* p, long long ld);
-void tcg_set_rowvec_ld(TcgPlan* p, long long ld);
 }
 using namespace b200;
 
@@ -111,7 +110,7 @@ struct b200_ncsnpp {
   std::vector<Op> ops;
   // Two half-batch "lanes" (ops2 = the second half's plan, empty when the batch is not split).  The lanes are
   // independent within one network evaluation, so forward() issues them on two streams: while one lane's
-  // HBM-bound GroupNorm/FIR pass streams, the other lane's tcgen05 contraction owns the tensor pipes.
+  // HBM-bound GroupNorm/FIR pass streams, the other lane's tensor-core contraction owns the tensor pipes.
   std::vector<Op> ops2;
   int B0 = 0;                                  // images in lane 0 (lane 1 holds B - B0)
   cudaStream_t lane_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -119,7 +118,6 @@ struct b200_ncsnpp {
 
   std::vector<TcGemmPlan*> tcplans;
   std::vector<TcAttnPlan*> attnplans;
-  std::vector<TcgPlan*> tcgplans;
   std::map<int, Tensor> taps;
   long long launches = 0;
   // per-call arguments read by the closures
@@ -129,7 +127,6 @@ struct b200_ncsnpp {
   ~b200_ncsnpp() {
     for (auto* p : tcplans) tc_gemm_plan_destroy(p);
     for (auto* p : attnplans) tc_attn_plan_destroy(p);
-    for (auto* p : tcgplans) tcg_plan_destroy(p);
     if (lane_stream) cudaStreamDestroy(lane_stream);
     if (ev_fork) cudaEventDestroy(ev_fork);
     if (ev_join) cudaEventDestroy(ev_join);
@@ -307,7 +304,7 @@ int build_graph(b200_ncsnpp* e) {
       }
       if (c.progressive_input == 1) {
         Mod m; m.kind = M_PYR_DOWN; m.index = cur(); m.cin1 = pyr_ch; m.cout = in_ch; m.res = all_res[lvl];
-        // FIR-padded stride-2 VALID conv: on tcgen05 via TMA element strides when the channel counts tile
+        // FIR-padded stride-2 VALID conv: on the tensor cores via TMA element strides when the channel counts tile
         m.tc0 = tc_ok(e, pyr_ch, 0, in_ch, all_res[lvl] / 2, all_res[lvl] / 2, 9);
         // image-channel pyramid level (3 channels): im2col patches + one K=32 contraction, like the input conv
         m.tc2 = tcmode && (9 * pyr_ch <= 32) && tc_ok(e, flatk, 0, in_ch, all_res[lvl] / 2, all_res[lvl] / 2, 1);
@@ -352,7 +349,7 @@ int build_graph(b200_ncsnpp* e) {
     // ([9][128][in_ch]; bias padded likewise), run as a swapped-operand convolution whose epilogue stores only those
     // rows, as NCHW, divided by sigma.  2.3x faster than the CUDA-core head despite the 125 idle rows.
     // cfg.cuda_core_head = 1 keeps the head on CUDA cores with an fp32 input (it is the one convolution with no later
-    // layer to average its operand rounding: +1e-4 of the parity budget on tensor cores, DESIGN.md section 2).
+    // layer to average its operand rounding: +1e-4 of the parity budget on tensor cores).
     m.tc0 = !c.cuda_core_head && tcmode && ch <= 32 && tc_ok(e, in_ch, 0, 128, c.image_size, c.image_size, 9) && (c.image_size * c.image_size) % 256 == 0 &&
             (c.image_size <= 128 || c.image_size % 128 == 0);
     m.w = m.tc0 ? add_param(e, nm("weight"), {ch, in_ch, 3, 3}, PK_CONV_PAD128, 9, ch, in_ch, om, -1, 9LL * 128 * in_ch)
@@ -377,7 +374,6 @@ struct Builder {
   b200_ncsnpp* e; int B; char* base; bool dry; Arena arena; int rc = 0;
   char* stats_base = nullptr; long long stats_top = 0;   // bump region for GroupNorm quad sums, zeroed once per forward
   bool fused_stats = false;
-  bool gn_on_load = false;                     // GroupNorm+SiLU applied by the consuming convolution (gemm_tcg.cuh) where shapes allow
   bool lowc_gn = false;                        // the few-channel convolutions (conv_lowc.cu, TF32 mode) apply GroupNorm+SiLU while staging their input
   int lane = 0;                                // which half-batch plan this builder fills (ops or ops2)
   int om = 1;                                  // operand store mode of tensor-core inputs: 1 TF32-grid fp32, 2 fp16
@@ -389,7 +385,6 @@ struct Builder {
   Builder(b200_ncsnpp* e_, int B_, char* base_, bool dry_, int lane_ = 0) : e(e_), B(B_), base(base_), dry(dry_), arena(e_->cfg.keep_activations != 0), lane(lane_) {
     fused_stats = e_->cfg.precision != 1;
     om = e_->cfg.precision == 2 ? 2 : 1;
-    gn_on_load = om == 2 && e_->cfg.separate_groupnorm == 0;
     lowc_gn = e_->cfg.precision == 0 && e_->cfg.separate_groupnorm != 2;
     if (dry_) stats_base = reinterpret_cast<char*>(uintptr_t(1) << 40);   // any non-null base: only offsets matter in a dry run
   }
@@ -414,16 +409,16 @@ struct Builder {
   void tfree(Tensor& t) { if (t.p) arena.release((char*)t.p - base, t.bytes); t.p = nullptr; }
   void ffree(float* p, long long bytes) { arena.release((char*)p - base, bytes); }
 
-  // kind: 0 tcgen05 contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc
+  // kind: 0 tensor-core contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc
   void op(int launches, std::function<int(cudaStream_t)> f, int kind = 6, double flops = 0.0) {
     if (dry) return;
     e->launches += launches;
-    static const char* kind_names[] = {"tcgen05", "cuda-core contraction", "groupnorm", "fir", "softmax", "time embedding", "misc", "mma.sync contraction"};
+    static const char* kind_names[] = {"tensor-core contraction", "cuda-core contraction", "groupnorm", "fir", "softmax", "time embedding", "misc", "mma.sync contraction"};
     (lane ? e->ops2 : e->ops).push_back({kind, flops, std::move(f), next_name.empty() ? std::string(kind_names[kind & 7]) : next_name, next_bytes});
     next_name.clear(); next_bytes = 0.0;
   }
 
-  // make sure tensor t has quad sums: produced by its tcgen05 epilogue, else by one streaming pass
+  // make sure tensor t has quad sums: produced by its tensor-core epilogue, else by one streaming pass
   void ensure_qs(Tensor& t) {
     if (t.qs || !t.p) return;
     t.qs = qalloc(t.C);
@@ -453,15 +448,7 @@ struct Builder {
     }, 2);
   }
 
-  // ---- GroupNorm on load (gemm_tcg.cuh): coefficient tables + the convolution that consumes them ----
-  bool tcg_shape_ok(int C1, int C2, int Cout, int H, int W, int C3 = 0, int C4 = 0) const {
-    if (!gn_on_load || !fused_stats) return false;
-    TcgDesc d; memset(&d, 0, sizeof(d));
-    d.a1 = (const void*)16; d.C1 = C1; d.a2 = C2 ? (const void*)16 : nullptr; d.C2 = C2;
-    d.a3 = C3 ? (const void*)16 : nullptr; d.C3 = C3; d.a4 = C4 ? (const void*)16 : nullptr; d.C4 = C4; d.w2 = C3 ? (const float*)16 : nullptr;
-    d.H = H; d.W = W; d.nimg = 1; d.N_total = Cout; d.epi.ld_out = Cout; d.epi.ld_res = Cout; d.epi.rows_per_img = H * W;
-    return tcg_supported(d, nullptr);
-  }
+  // ---- GroupNorm coefficient tables for the few-channel convolutions that normalise while staging their input ----
   struct Coef { float* scale = nullptr; float* shift = nullptr; long long bytes = 0; };
   Coef gncoef(Tensor& x1, Tensor& x2, int pgw, int pgb) {
     const int C = x1.C + x2.C, G = std::min(C / 4, 32), HW = x1.H * x1.W;
@@ -474,43 +461,6 @@ struct Builder {
     op(1, [=](cudaStream_t st) { return launch_gn_coeff(a.C, b.C, a.qs, b.qs, g, bt, Bc, HW, G, 1e-6f, cc.scale, cc.shift, st); }, 2);
     return c;
   }
-  // out = epi(Conv3x3(SiLU(GN(cat[a1, a2]))) [+ Conv1x1(cat[x3, x4])]); a*/x* are read in their stored format (fp32 or fp16)
-  void convg(Tensor a1, Tensor a2, const Coef& cf, int pw, int pb, int Cout, int dense_row, const float* residual, float scale,
-             int round, Tensor& out, Tensor x3 = Tensor(), Tensor x4 = Tensor(), int pw2 = -1, int pb2 = -1) {
-    TcgDesc d; memset(&d, 0, sizeof(d));
-    d.a1 = a1.p; d.C1 = a1.C; d.a1_f16 = a1.f16; d.a2 = a2.p; d.C2 = a2.C; d.a2_f16 = a2.f16;
-    d.gn_scale = cf.scale; d.gn_shift = cf.shift; d.act = 1;
-    d.H = out.H; d.W = out.W; d.nimg = B; d.w = e->W(pw); d.N_total = Cout;
-    Epilogue ep; memset(&ep, 0, sizeof(ep));
-    ep.bias = e->W(pb); ep.residual = residual; ep.ld_res = Cout; ep.scale = scale; ep.round_tf32 = round;
-    ep.rows_per_img = out.H * out.W; ep.out = out.p; ep.ld_out = Cout;
-    if (dense_row >= 0) ep.rowvec = dense_all_ + dense_row;
-    if (x3.p) {
-      if (dense_row >= 0) { set_error("ncsnpp: fused skip projection on a conv with a time-embedding bias"); rc = 2; return; }
-      d.a3 = x3.p; d.C3 = x3.C; d.a3_f16 = x3.f16; d.a4 = x4.p; d.C4 = x4.C; d.a4_f16 = x4.f16; d.w2 = e->W(pw2);
-      ep.rowvec = e->W(pb2); ep.rowvec_ld = 0;
-    }
-    if (fused_stats) { out.qs = qalloc(Cout); d.qstats = out.qs; }
-    d.epi = ep;
-    if (dry) return;
-    TcgPlan* pl = nullptr;
-    if (int r = tcg_plan_create(d, &pl)) { rc = r; return; }
-    e->tcgplans.push_back(pl);
-    name("conv3x3 gn+silu %d+%d->%d @%d%s%s [pair256-gn]", a1.C, a2.C, Cout, out.H, x3.p ? " +skipproj" : "", residual ? " +res" : "");
-    if (x3.p) next_name += " " + std::to_string(x3.C + x4.C);
-    {
-      const double px = (double)B * out.H * out.W;
-      next_bytes = px * (a1.C * (a1.f16 ? 2.0 : 4.0) + a2.C * (a2.f16 ? 2.0 : 4.0) + x3.C * (x3.f16 ? 2.0 : 4.0) + x4.C * (x4.f16 ? 2.0 : 4.0)) +
-                   px * Cout * (round == 2 ? 2.0 : 4.0) + (residual ? px * Cout * 4.0 : 0.0) + (9.0 * (a1.C + a2.C) + x3.C + x4.C) * Cout * 2.0;
-    }
-    b200_ncsnpp* eng = e; const int sumC = e->sumC;
-    const double cflops = 2.0 * B * out.H * out.W * (double)Cout * ((a1.C + a2.C) * 9 + x3.C + x4.C);
-    op(1, [=](cudaStream_t st) {
-      if (dense_row >= 0) tcg_set_rowvec_ld(pl, eng->uniform ? 0 : sumC);
-      return tcg_launch(pl, st);
-    }, 0, cflops);
-  }
-
   // 2x resampling of a resblock (layerspp.py:244-256).  fir=True: upsample_2d / downsample_2d with the configured FIR
   // (up_or_down_sampling.py:218-224, 252-257); fir=False: naive_upsample_2d (nearest-neighbour repeat) and
   // naive_downsample_2d (2x2 mean) (:59-69), expressed as the same upfirdn2d with a 2x2 box: up=2, pad (1,0), taps 1
@@ -560,7 +510,7 @@ struct Builder {
     const int sumC = e->sumC;
     const double cflops = 2.0 * B * out.H * out.W * (double)Cout * ((a1.C + a2.C) * taps + x3.C + x4.C);
     if (x3.p && !use_tc) { set_error("ncsnpp: fused skip projection needs the tensor-core path"); rc = 2; return; }
-    if (gnc && use_tc) { set_error("ncsnpp: conv(): GroupNorm coefficients go with the few-channel kernel (convg() is the tcgen05 form)"); rc = 2; return; }
+    if (gnc && use_tc) { set_error("ncsnpp: conv(): GroupNorm coefficients go with the few-channel kernel (the tensor-core path reads normalised operands)"); rc = 2; return; }
     if (use_tc) {
       TcGemmDesc d; memset(&d, 0, sizeof(d));
       d.a1 = a1.p; d.C1 = a1.C; d.a2 = a2.p; d.C2 = a2.C; d.conv = 1; d.H = out.H; d.W = out.W; d.nimg = B; d.taps = taps;
@@ -622,7 +572,7 @@ struct Builder {
   void gemm(bool use_tc, const float* A, long long lda, long long a_rows, int a_batch_rows, const float* Wm, long long ldw,
             long long w_rows, int w_batch_rows, int nbatch, int M, int N, int K, const float* bias,
             const float* residual, long long ld_res, float scale, int round, float* out, long long ldo,
-            double* qstats = nullptr, int rows_per_img = 1 << 30, bool no_pair = false) {
+            double* qstats = nullptr, int rows_per_img = 1 << 30) {
     Epilogue ep; memset(&ep, 0, sizeof(ep));
     ep.bias = bias; ep.residual = residual; ep.ld_res = ld_res; ep.scale = scale; ep.round_tf32 = round;
     ep.rows_per_img = rows_per_img; ep.out = out; ep.ld_out = ldo;
@@ -630,7 +580,7 @@ struct Builder {
       TcGemmDesc d; memset(&d, 0, sizeof(d));
       d.a1 = A; d.C1 = K; d.conv = 0; d.taps = 1; d.a_rows = a_rows; d.a_ld = lda; d.a_batch_rows = a_batch_rows;
       d.w = Wm; d.N_total = N; d.K_total = K; d.w_rows = w_rows; d.w_ld = ldw; d.w_batch_rows = w_batch_rows;
-      d.nbatch = nbatch; d.M_per_batch = M; d.qstats = qstats; d.no_pair = no_pair ? 1 : 0; d.epi = ep;
+      d.nbatch = nbatch; d.M_per_batch = M; d.qstats = qstats; d.epi = ep;
       d.f16 = om == 2;
       if (dry) return;
       TcGemmPlan* pl = nullptr;
@@ -670,13 +620,7 @@ struct Builder {
     const int Cin = x1.C + x2.C, H = x1.H, Ho = m.up ? 2 * H : m.down ? H / 2 : H;
     const bool resample = m.up || m.down;
     const float inv_s2 = e->cfg.skip_rescale ? 1.0f / (float)std::sqrt(2.0) : 1.0f;
-    // GroupNorm on load (fp16 operand mode, 256-channel outputs at 16x16 / 32x32): GroupNorm_1 + SiLU is applied by Conv_1
-    // while it builds its operand (g1), GroupNorm_0 + SiLU by Conv_0 when no FIR resampling sits in between (g0).  The
-    // skip projection then reads the block input itself (fp32 -> fp16 on load), so no rounded copy is written either.
     const bool h1_f16 = om == 2 && m.tc0 && m.tc1 && fused_stats && (Ho * Ho) % 32 == 0 && (m.cout % 128 == 0);
-    const bool skip_ok = !m.has_conv2 || (m.tc2 && (resample ? Cin % 64 == 0 : (x1.C % 64 == 0 && x2.C % 64 == 0)));
-    const bool g1 = m.tc0 && m.tc1 && h1_f16 && skip_ok && tcg_shape_ok(m.cout, 0, m.cout, Ho, Ho);
-    const bool g0 = g1 && !resample && tcg_shape_ok(x1.C, x2.C, m.cout, Ho, Ho);
     // few-channel levels (TF32 mode): both 3x3 convolutions normalise their input while they stage it, so neither
     // GroupNorm writes a tensor (quad-aligned groups only: the coefficient kernel works on channel quads)
     const int G0 = std::min(Cin / 4, 32);
@@ -684,9 +628,9 @@ struct Builder {
                      lowc_ok(x1.C, x2.C, m.cout, H, 9);
     const bool lc1 = lowc_gn && !m.tc1 && lowc_ok(m.cout, 0, m.cout, Ho, 9);
     Tensor a0, raw;   // raw: operand-format copy of the (concatenated) block input for the tensor-core skip conv
-    if (!g0 && !lc0) {
+    if (!lc0) {
       a0 = talloc(Cin, H, H);
-      if (m.has_conv2 && m.tc2 && !resample && !g1) raw = talloc(Cin, H, H);
+      if (m.has_conv2 && m.tc2 && !resample) raw = talloc(Cin, H, H);
       gn(x1, x2, m.gn0w, m.gn0b, 1, (m.tc0 && !resample) ? om : 0, a0, raw.p);
     }
     Tensor xr;
@@ -703,11 +647,7 @@ struct Builder {
     // fp16 operand mode: the mid-block tensor (Conv_0 output, only ever read by GroupNorm_1) is stored as fp16;
     // its GroupNorm sums are accumulated from the fp32 accumulators in the epilogue.
     h1.f16 = h1_f16;
-    if (g0) {
-      Coef c0 = gncoef(x1, x2, m.gn0w, m.gn0b);
-      convg(x1, x2, c0, m.c0w, m.c0b, m.cout, m.dense_row, nullptr, 1.f, 2, h1);
-      ffree(c0.scale, c0.bytes);
-    } else if (lc0) {
+    if (lc0) {
       Coef c0 = gncoef(x1, x2, m.gn0w, m.gn0b);
       conv(false, x1, x2, 9, m.c0w, m.c0b, m.cout, m.dense_row, nullptr, 1.f, 0, h1, /*want_stats=*/true, 1, 0, Tensor(), Tensor(), -1, -1, &c0);
       ffree(c0.scale, c0.bytes);
@@ -716,19 +656,6 @@ struct Builder {
       tfree(a0);
     }
     if (h1_f16 && !h1.qs) { set_error("ncsnpp: fp16 mid-block tensor without fused GroupNorm sums"); rc = 2; return Tensor(); }
-    if (g1) {
-      Coef c1 = gncoef(h1, none, m.gn1w, m.gn1b);
-      Tensor out = talloc(m.cout, Ho, Ho);
-      if (m.has_conv2) {
-        if (resample) convg(h1, none, c1, m.c1w, m.c1b, m.cout, -1, nullptr, inv_s2, 0, out, xr, Tensor(), m.c2w, m.c2b);
-        else convg(h1, none, c1, m.c1w, m.c1b, m.cout, -1, nullptr, inv_s2, 0, out, x1, x2, m.c2w, m.c2b);
-      } else {
-        convg(h1, none, c1, m.c1w, m.c1b, m.cout, -1, x1.p, inv_s2, 0, out);
-      }
-      ffree(c1.scale, c1.bytes);
-      tfree(h1); tfree(xr);
-      return out;
-    }
     Tensor a1; Coef c1;
     if (lc1) {
       c1 = gncoef(h1, none, m.gn1w, m.gn1b);
@@ -805,7 +732,7 @@ struct Builder {
       // q,k = a Wq^T + bq | a Wk^T + bk   (layerspp.py:78-79) in one N=2C contraction
       gemm(tc, a.p, C, BT, 0 /* rows enumerated flat */, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, bqkv, nullptr, 0, 1.f, tc ? om : 0, qk, 2 * C);
       // v^T[b][c][t] = sum_i Wv[c][i] a[b][t][i]   (bias bv is added after the PV product: softmax rows sum to 1)
-      gemm(tc, wv, C, C, 0, a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, vT, T, nullptr, 1 << 30, /*no_pair=*/true);
+      gemm(tc, wv, C, C, 0, a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, vT, T, nullptr, 1 << 30);
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
       // [T,T] logits/probabilities and the attention output stay on chip; other token counts (tf32 mode) use separate launches.
@@ -831,7 +758,7 @@ struct Builder {
       }
       float* S = falloc(BT * T, &sb);
       // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax
-      gemm(tc, qk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30, /*no_pair=*/true);
+      gemm(tc, qk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30);
       ffree(qk, qkb);
       name("softmax T=%d", T);
       op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
@@ -890,7 +817,7 @@ struct Builder {
       const Mod& m = e->mods[mi++];
       Tensor h0 = talloc(nf, R, R);
       if (m.tc0 || m.tc1) {
-        // im2col patches [B*R*R][32] (TF32 grid) then one K=32 contraction with the flat-packed weights (tcgen05, or the
+        // im2col patches [B*R*R][32] (TF32 grid) then one K=32 contraction with the flat-packed weights (tensor cores, or the
         // few-channel kernel for nf <= 64)
         long long pb; float* patches = falloc((long long)B * R * R * 32, &pb);   // 128 B per pixel: 32 fp32 or 64 fp16
         const int Bc = B, omc = om;
@@ -1123,6 +1050,8 @@ extern "C" {
 
 int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
   B200_REQUIRE(cfg && out, "ncsnpp_create: null argument");
+  B200_REQUIRE(cfg->separate_groupnorm != 0, "ncsnpp_create: separate_groupnorm = 0 (GroupNorm applied on load by the tensor-core "
+               "convolution) is not available in this build; use 1 or 2");
   b200_ncsnpp* e = new b200_ncsnpp();
   e->cfg = *cfg;
   if (int r = build_graph(e)) { delete e; return r; }
@@ -1209,8 +1138,6 @@ int b200_ncsnpp_bind_workspace(b200_ncsnpp_t* h, int batch, void* ws, long long 
   for (auto* p : h->tcplans) tc_gemm_plan_destroy(p);
   for (auto* p : h->attnplans) tc_attn_plan_destroy(p);
   h->attnplans.clear();
-  for (auto* p : h->tcgplans) tcg_plan_destroy(p);
-  h->tcgplans.clear();
   h->tcplans.clear(); h->ops.clear(); h->ops2.clear(); h->taps.clear(); h->launches = 0;
   h->B = batch; h->ws_bytes = ws_bytes;
   h->ws = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~uintptr_t(1023));

@@ -1,36 +1,30 @@
-// tcgen05 / TMEM / TMA implicit GEMM for the NCSN++ contractions (3x3 and 1x1
-// convolutions, NIN projections, the attention products) on sm_100a.
+// wgmma / TMA implicit GEMM for the NCSN++ contractions (3x3 and 1x1 convolutions, NIN projections, the attention
+// products) on sm_90a.
 //
 //   out[b][m, n] = epi( sum_{src, tap, c} A_src(b, m, tap, c) * W(b)[tap][n][koff_src + c]
 //                       (+ an optional extra 1x1 phase: the fused skip projection) )
 //
-// Operands are written by their producers in the contraction's format: fp32 bit patterns
-// rounded to the TF32 grid (kind::tf32, 32 channels per 128-byte K step) or IEEE fp16
-// (kind::f16, 64 channels per K step); either way 11 significand bits, fp32 accumulation in TMEM.
+// Operands are written by their producers in the contraction's format: fp32 bit patterns rounded to the TF32 grid
+// (wgmma .tf32, 32 channels per 128-byte K step) or IEEE fp16 (wgmma .f16, 64 channels per K step); either way 11
+// significand bits, fp32 accumulation in registers.
 //
-// Kernels (persistent, warp-specialised, 384 threads unless noted):
-//   gemm_tc_kernel<BN, STAGES, false>  one CTA per tile: 128 rows x BN columns, or - `swap` - 128 output
-//                                      channels x 256 pixels (D^T = W X^T) for 128-channel convolutions,
-//                                      1x1 convolutions and the network head;
-//   gemm_tc2_kernel<BN, STAGES>        gemm_tc2.cuh: a CTA pair (cta_group::2) per 256-row tile, each CTA
-//                                      stages its own A rows and half of the W tile;
-//   attn_tc_kernel<F16>                attn_tc.cuh: QK^T, softmax, PV, NIN_3 + residual in one kernel;
-//   gemm_tc_kernel<BN, STAGES, true>   256 threads: the smem-staged TMA-store epilogue kept for A/B runs.
+// Kernels (persistent, warp-specialised, 384 threads):
+//   gemm_tc_kernel<BN>   one CTA per tile: 128 rows x BN columns, or - `swap` - 128 output channels x 256 pixels
+//                        (D^T = W X^T) for 128-channel convolutions, 1x1 convolutions and the network head;
+//   attn_tc_kernel<F16>  attn_tc.cuh: QK^T, softmax, PV, NIN_3 + residual in one kernel.
 // Roles: warp 0 TMA producer (4-D box of the NHWC tensor shifted by the filter tap - or, in the halo form, three
 // W-shifted copies of the tile with its halo per channel chunk - zero halo and tail rows from out-of-bounds fill,
-// SWIZZLE_128B, ring with full/empty mbarriers); warp 1 MMA issuer (four MMAs per K step into one of two TMEM
-// accumulator stages, tcgen05.commit frees the slot / publishes the accumulator); both run as WHOLE warps whose
-// loop state is warp-uniform, with the TMA / tcgen05 instructions predicated on one elect.sync lane (see elect_one:
-// under a `lane == 0` branch every such instruction was wrapped in a lane-serialising loop and the issue loop became
-// the bound of the kernel); warp 2 TMEM allocation; warps 4..11 epilogue, two per TMEM lane
-// quarter: tcgen05.ld, then a block routine compiled per (residual, store format, stats) combination -
-// `row_chunk_t` (row-major outputs: 32x32 blocks transposed through warp-private shared memory so global
-// accesses are coalesced) or `swap_chunk` (lane = channel, already coalesced) - with bias, time-embedding
-// row, residual, scale, fp32 / TF32 / fp16 store and the GroupNorm quad sums fused.
+// SWIZZLE_128B, ring with full/empty mbarriers), running as a whole warp with warp-uniform loop state and the TMA
+// instructions predicated on one elect.sync lane; warps 1..3 idle (their registers go to the MMA warpgroups);
+// warps 4..11 two MMA warpgroups, each issuing m64 x BN wgmma over its 64 rows of the tile and then storing its
+// accumulator fragment through an epilogue compiled per (residual, store format, stats) combination - `frag_rows`
+// (row-major outputs) or `frag_swap` (swapped tiles) - with bias, time-embedding row, residual, scale,
+// fp32 / TF32 / fp16 store and the GroupNorm quad sums fused.
 #include "kernels.h"
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
+#include "wgmma.cuh"
 #include <mutex>
 #include <cstdlib>
 #include <cstring>
@@ -39,19 +33,17 @@ namespace b200 {
 
 namespace {
 
-constexpr int BM = 128;          // rows (pixels) per tile == UMMA M
+constexpr int BM = 128;          // rows (pixels) per tile: two m64 warpgroup tiles
 constexpr int BKE = 32;          // fp32 elements per K step == one 128-byte swizzle row
 constexpr int A_STAGE_BYTES = BM * BKE * 4;   // 16 KiB
 
-// Halo form of the 3x3 mainloop (DESIGN.md section 4.13).  The nine filter taps of one channel chunk read three W-shifted
+// Halo form of the 3x3 mainloop.  The nine filter taps of one channel chunk read three W-shifted
 // copies of the tile *with its one-row halo* (TMA box [chunk, W, rows + 2], origin w = -1 / 0 / +1, zero fill outside the
 // image); the operand of tap (dh, dw) is copy[dw] starting (dh + 1) * W pixels in - a multiple of 1024 bytes, so a plain
 // swizzled descriptor.  L2 -> shared-memory traffic per chunk: 3 x (rows + 2) / rows tiles instead of 9.
-constexpr int HALO_XS = 4;                  // halo copies in flight (both kernels)
-constexpr int HALO_X_BYTES = 40 * 1024;     // single-CTA swapped form: (8 + 2) rows x 32 pixels x 128 B
-constexpr int HALO_WS = 4;                  //   its weight-slice ring: 4 x 16 KB   (4 x 40 + 4 x 16 = 224 KB = the plain form's footprint)
-constexpr int HALO2_X_BYTES = 24 * 1024;    // CTA pair: (4 + 2) rows x 32 pixels x 128 B per CTA
-constexpr int HALO2_WS = 6;                 //   its weight-half ring: 6 x 16 KB   (4 x 24 + 6 x 16 = 192 KB = the plain form's stages)
+constexpr int HALO_XS = 4;                  // halo copies in flight
+constexpr int HALO_X_BYTES = 40 * 1024;     // swapped form: (8 + 2) rows x 32 pixels x 128 B
+constexpr int HALO_WS = 4;                  //   its weight-slice ring: 4 x 16 KB   (4 x 40 + 4 x 16 = 224 KB)
 
 struct TcParams {
   CUtensorMap tmA1, tmA2, tmW;
@@ -61,14 +53,14 @@ struct TcParams {
   int halo_dh_bytes;                       // W * 128: bytes between the operand windows of consecutive filter rows inside a copy
   int halo_copy_bytes;                     // (tile rows + 2) * W * 128: bytes of one halo copy
   int halo_prefetch;                       // 1: the halo producers prefetch the next tile's halo boxes (all channel chunks) into L2 (opt-in: measured -2 %)
-  int chunk_major;                         // nine-load loop of the single-CTA kernel walks K as (chunk, filter column, filter row): shapes with a halo form
+  int chunk_major;                         // nine-load loop walks K as (chunk, filter column, filter row): shapes with a halo form
   int conv, H, W, taps, pad, S, stride;   // H, W: OUTPUT spatial size; S = filter width (3 or 1)
   int kchunks1, kchunks2, C1;
   int kchunks3, kchunks4, C3;              // extra phase: channel chunks of its (two-source) input
   int N_total, tiles_n;
   int nbatch, tiles_m_per_batch, M_per_batch;
   int a_batch_rows, w_batch_rows;
-  int f16;                                 // 1: A and W are fp16 (tcgen05 kind::f16, 64-channel K steps); 0: TF32-grid fp32 (32-channel K steps)
+  int f16;                                 // 1: A and W are fp16 (wgmma .f16, 64-channel K steps); 0: TF32-grid fp32 (32-channel K steps)
   int bke;                                 // channels per K step: one 128-byte swizzle row = 32 fp32 or 64 fp16
   int swap;                                // 1: operands swapped (D^T = W X^T): 128 output channels x 256 pixels per tile
   double* qstats;                          // optional [img][N_total/4][2] GroupNorm quad sums (sum, sum of squares)
@@ -99,15 +91,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must surface as a trapped kernel (launch error), never as a hung GPU.
+// Bounded wait: a protocol bug must surface as a trapped kernel (launch error), never as a hung GPU.  (No printf here:
+// a call anywhere in a kernel makes ptxas serialise its wgmma pipeline.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {   // ~4 s at 2 GHz
-      printf("gemm_tc: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 8000000000LL) __trap();   // ~4 s at 2 GHz
   }
 }
 
@@ -130,353 +120,302 @@ __device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* tm, int c0, i
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// Pull one 128-byte line towards L2 without occupying a register: the epilogues use it for their residual rows
-// while they still wait for the accumulator, so the later loads hit L2 instead of paying an HBM round trip
-// inside the per-chunk critical path (the 112-register cap that lets GroupNorm CTAs co-reside leaves no room
-// for a register-held prefetch).
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
-// Explicit shared-space 128-bit accesses.  Through a generic pointer the compiler emitted LD.E / ST.E for the
-// epilogue's transposition scratch (it cannot prove the address space of a pointer derived from the dynamic smem
-// base), i.e. long-scoreboard loads that it then serialised one row at a time: the attention kernel's `final`
-// phase spent most of its samples waiting on them (profiles/r01_c31_ncu_attn_tc_f16.md).
-__device__ __forceinline__ float4 lds128(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+// K-major, 128-byte-swizzled operand tile (rows of 128 B, 8-row atoms 1024 B apart) as an sm_90 wgmma descriptor:
+// start address >> 4, LBO 16 B (unused for swizzled K-major), SBO 1024 B, layout type 1 = SWIZZLE_128B.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// the four MMAs of one 128-byte K step: 4 x K=8 (tf32) or 4 x K=16 (f16); either way +32 B per slice
-template <bool F16>
-__device__ __forceinline__ void umma_kstep(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, int it) {
+// One 128-byte K step of an m64nN tile: 4 x K=8 (tf32) or 4 x K=16 (f16); either way +32 B per slice (+2 in the
+// descriptor's address field).  `it` counts K steps of the tile: the first one overwrites the accumulator.
+template <int N, bool F16>
+__device__ __forceinline__ void wgmma_kstep(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, int it) {
+  wgmma_fence();
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    // advance 32 B along K inside the 128-B swizzle row: +2 in the (addr>>4) field
-    if (F16) umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (it | k) != 0);
-    else umma_tf32(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (it | k) != 0);
+    const uint32_t acc = (it | k) != 0;
+    if constexpr (F16) {
+      if constexpr (N == 256) wgmma_f16_n256(d, adesc + 2 * k, bdesc + 2 * k, acc);
+      else wgmma_f16_n128(d, adesc + 2 * k, bdesc + 2 * k, acc);
+    } else {
+      if constexpr (N == 256) wgmma_tf32_n256(d, adesc + 2 * k, bdesc + 2 * k, acc);
+      else wgmma_tf32_n128(d, adesc + 2 * k, bdesc + 2 * k, acc);
+    }
   }
+  wgmma_commit();
 }
-// One lane of a converged warp (elect.sync).  The MMA issuer runs as a whole warp with its loop counters, barrier
-// addresses and descriptors warp-uniform, and only the tcgen05 instructions predicated on this: under a `lane == 0`
-// branch the compiler cannot prove a single active lane and wraps every UTCHMMA / UTCBAR in an ELECT / R2UR.BROADCAST /
-// BRA.U.ANY loop (~8 extra instructions per MMA), which made the issue loop - not data, not the tensor pipe - the
-// bound of every convolution (profiles/r02_h1_ncu_swap_halo.md: the issuer's samples sit on ALU latencies, DESIGN.md 4.13).
+
+// One lane of a converged warp (elect.sync): the producer runs as a whole warp with warp-uniform loop state and only
+// the TMA instructions predicated on this.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows are 128 B, 8-row atoms are 1024 B apart.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  const uint64_t lo = (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16);            // start address, LBO (unused for swizzled K-major)
-  const uint64_t hi = (uint64_t)(1024 >> 4) | (1ull << 14) | (2ull << 29);           // SBO = 1024 B, version 1 (sm_100), SWIZZLE_128B
-  return lo | (hi << 32);
-}
+// Register budget of the warp-specialised kernels (384 threads, one CTA per SM): the producer warpgroup gives its
+// registers to the two MMA warpgroups, whose m64n256 fp32 accumulators take 128 registers per thread.
+__device__ __forceinline__ void regs_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void regs_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+__device__ __forceinline__ void wg_barrier(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }
 
 template <int BN>
-__host__ __device__ constexpr uint32_t make_idesc() {
-  // D fp32 (1<<4), A tf32 (2<<7), B tf32 (2<<10), both K-major, N>>3 at bit 17, M>>4 at bit 24.
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-template <int BN>
-__host__ __device__ constexpr uint32_t make_idesc_f16() {
-  // kind::f16: D fp32 (1<<4), A fp16 (0<<7), B fp16 (0<<10)
-  return (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
-
-template <int BN, int STAGES>
 struct SmemLayout {
+  static constexpr int STAGES = BN == 256 ? 4 : 6;
   static constexpr int B_STAGE_BYTES = BN * BKE * 4;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int TRN_OFFSET = STAGES * STAGE_BYTES;   // 8 epilogue warps x 4 KB transposition scratch
-  static constexpr int BAR_OFFSET = TRN_OFFSET + 8 * 4096;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int HALO_BYTES = HALO_XS * HALO_X_BYTES + HALO_WS * A_STAGE_BYTES;   // the swapped halo form's two rings
+  static constexpr int BAR_OFFSET = BN == 256 && HALO_BYTES > RING_BYTES ? HALO_BYTES : RING_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // barriers + slack for 1024-B alignment
-  static_assert(TOTAL <= 232448, "exceeds the 227 KB shared-memory limit of sm_100");
+  static_assert(TOTAL <= 232448, "exceeds the 227 KB shared-memory limit of sm_90");
+  static_assert(BN != 256 || STAGES >= HALO_XS, "the halo copies use the first HALO_XS stage barriers");
 };
 
-// GroupNorm quad sums of one 32-column chunk held one row per lane.  st[0..7] = per-quad sums of the lane's
-// row, st[8..15] = per-quad sums of squares (zeros for rows past the end).  Halving butterfly: each exchange
-// sends half of the live entries to the partner lane and adds the partner's other half, so after four
-// exchanges a lane holds ONE entry summed over 16 lanes (16 shuffles instead of 80); a final exchange
-// completes the 32-row sum.  rows_per_img == 16 (4x4 images): the two half-warps are different images and are
-// reduced separately.  The entry totals are then accumulated in fp64 by 16 (or 32) lanes in parallel.
-__device__ __forceinline__ void quad_stats_commit_raw(double* qstats, int n_total, int rows_per_img, float (&st)[16],
-                                                      int img, bool valid, int col0, int lane) {
-  const bool halves = rows_per_img < 32;
-  int idx = 0;
-  if (!halves) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const bool up = lane & 16;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 8], 16);
-      st[i] = (up ? st[i + 8] : st[i]) + recv;
-    }
-    idx = (lane & 16) ? 8 : 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const bool up = lane & 8;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 4], 8);
-      st[i] = (up ? st[i + 4] : st[i]) + recv;
-    }
-    idx += (lane & 8) ? 4 : 0;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const bool up = lane & 4;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 2], 4);
-      st[i] = (up ? st[i + 2] : st[i]) + recv;
-    }
-    idx += (lane & 4) ? 2 : 0;
-    {
-      const bool up = lane & 2;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[0] : st[1], 2);
-      st[0] = (up ? st[1] : st[0]) + recv;
-    }
-    idx += (lane & 2) ? 1 : 0;
-    st[0] += __shfl_xor_sync(0xffffffffu, st[0], 1);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const bool up = lane & 8;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 8], 8);
-      st[i] = (up ? st[i + 8] : st[i]) + recv;
-    }
-    idx = (lane & 8) ? 8 : 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const bool up = lane & 4;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 4], 4);
-      st[i] = (up ? st[i + 4] : st[i]) + recv;
-    }
-    idx += (lane & 4) ? 4 : 0;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const bool up = lane & 2;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[i] : st[i + 2], 2);
-      st[i] = (up ? st[i + 2] : st[i]) + recv;
-    }
-    idx += (lane & 2) ? 2 : 0;
-    {
-      const bool up = lane & 1;
-      const float recv = __shfl_xor_sync(0xffffffffu, up ? st[0] : st[1], 1);
-      st[0] = (up ? st[1] : st[0]) + recv;
-    }
-    idx += (lane & 1) ? 1 : 0;
-  }
-  // image / validity of the (half-)warp's rows: taken from its first row
-  const int img_w = __shfl_sync(0xffffffffu, img, halves ? (lane & 16) : 0);
-  const bool val_w = __shfl_sync(0xffffffffu, (int)valid, halves ? (lane & 16) : 0) != 0;
-  const bool writer = halves ? true : ((lane & 1) == 0);
-  if (writer && val_w && st[0] != 0.f) {
-    const int quad = idx & 7, which = idx >> 3;          // which: 0 = sum, 1 = sum of squares
-    atomicAdd(qstats + ((long long)img_w * (n_total >> 2) + (col0 >> 2) + quad) * 2 + which, (double)st[0]);
-  }
-}
-__device__ __forceinline__ void quad_stats_commit(const TcParams& p, const Epilogue& e, float (&st)[16], int img,
-                                                  bool valid, int col0, int lane) {
-  quad_stats_commit_raw(p.qstats, p.N_total, e.rows_per_img, st, img, valid, col0, lane);
-}
-
-// One 32-pixel chunk of the swapped-operand epilogue (lane = output channel, v[i] = pixel i of the chunk), specialised
-// on what the launch needs so the per-element instruction stream is minimal: the profile of the first version
-// (profiles/r01_c19_ncu_swap_f16.md) showed the eight epilogue warps ISSUE-bound at ~40 instructions per element
-// (runtime-uniform branches, an IEEE divide path for an unused divisor, 64-bit index multiplies) - longer than the
-// fp16 main loop of a 128-channel convolution.  RES: add the residual; MODE 0 fp32 store, 1 TF32-rounded, 2 fp16.
-template <bool RES, int MODE>
-__device__ __forceinline__ void swap_chunk(const uint32_t (&v)[32], float add, float scale, float* out, const float* res,
-                                           long long ld_out, long long ld_res, float& ssum, float& ssq) {
-  float rr[32];
-  if (RES) {
-    const float* rp = res;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { rr[i] = __ldg(rp); rp += ld_res; }
-  }
-  float* op = out;                                        // MODE 2: `out` addresses fp16 elements, ld_out counts them
-  uint16_t* oh = reinterpret_cast<uint16_t*>(out);
-#pragma unroll
-  for (int i = 0; i < 32; ++i) {
-    float o = __uint_as_float(v[i]) + add;
-    if (RES) o += rr[i];
-    o *= scale;
-    if (MODE == 1) o = round_tf32(o);
-    if (MODE == 2) {
-      uint16_t h;
-      asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(o));
-      *oh = h; oh += ld_out;
-    } else { *op = o; op += ld_out; }
-    ssum += o; ssq = fmaf(o, o, ssq);
-  }
-}
-
-// One 32-row x 32-column block of the direct epilogue (row-major outputs), specialised like swap_chunk: RES residual
-// add, MODE store format (0 fp32, 1 TF32-rounded fp32, 2 fp16), STATS GroupNorm quad sums of the stored fp32 values.
-// tcgen05.ld hands each lane one accumulator ROW; storing from that layout touches 32 different 128-byte lines with
-// every 128-bit load/store (the in-step ncu capture of the +residual 256-channel convolution showed the eight
-// epilogue warps bound by L1 wavefronts, tensor pipe 48 % vs 70 % without the residual; measured A/B of the two
-// forms: 173 -> 153 us for that launch, -2.2 % per PC step, profiles/r01_c23_*).  So the warp first
-// transposes its 32x32 block through 4 KB of warp-private shared memory (XOR-swizzled 16-byte slots: conflict-free
-// both ways), after which lane l owns column quad l%8 of rows l/8, l/8+4, ...: eight consecutive lanes cover one
-// 128-byte line, a warp instruction covers 4 lines instead of 32, bias / time-embedding quads are loaded once per
-// chunk, and the GroupNorm quad sums need 2 shuffle steps instead of the 16-shuffle butterfly.
-//   gm0: global row of the block's first row; rows_valid: rows of the block inside the matrix (0..32);
-//   img0: image of the first row; rows of one block span two images only when rows_per_img == 16.
-template <bool RES, int MODE, bool STATS>
-__device__ __forceinline__ void row_chunk_t(const uint32_t (&v)[32], uint8_t* tbuf, const Epilogue& e, double* qstats, int n_total,
-                                            long long gm0, int rows_valid, int n0, int img0, int lane) {
-  const uint32_t tb = smem_u32(tbuf);
-#pragma unroll
-  for (int qd = 0; qd < 8; ++qd)
-    sts128(tb + lane * 128 + ((qd ^ (lane & 7)) << 4), v[4 * qd], v[4 * qd + 1], v[4 * qd + 2], v[4 * qd + 3]);
-  __syncwarp();
-  const int cq = lane & 7, r0 = lane >> 3, col = n0 + cq * 4;
-  const bool two_img = e.rows_per_img < 32;
-  float4 addA = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (e.bias) addA = __ldg(reinterpret_cast<const float4*>(e.bias + col));
-  float4 addB = addA;
-  if (e.rowvec) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(e.rowvec + img0 * e.rowvec_ld + col));
-    addA.x += t.x; addA.y += t.y; addA.z += t.z; addA.w += t.w;
-    if (two_img) {
-      const float4 u = __ldg(reinterpret_cast<const float4*>(e.rowvec + (img0 + 1) * e.rowvec_ld + col));
-      addB.x += u.x; addB.y += u.y; addB.z += u.z; addB.w += u.w;
-    } else addB = addA;
-  }
+// Epilogue of one warp's 16 x BN slice of a row-major accumulator (rows = pixels / tokens, columns = output channels),
+// straight from the wgmma fragment: lane l holds rows l/4 and l/4 + 8, column pairs 8j + 2(l%4); a quad of lanes writes
+// 32 contiguous bytes of a row.  Specialised like the rest of the epilogue code: RES residual add, MODE store format
+// (0 fp32, 1 TF32-rounded fp32, 2 fp16), STATS GroupNorm quad sums of the stored values.
+//   gm: global row of the slice's first row; rows_valid: rows of the 16 inside the matrix; n0: first column.
+// The 16 rows of a slice belong to one image (rows_per_img % 16 == 0 wherever per-image terms are used).
+template <int BN, bool RES, int MODE, bool STATS>
+__device__ __forceinline__ void frag_rows(const float (&d)[BN / 2], const Epilogue& e, double* qstats, int n_total,
+                                          long long gm, int rows_valid, int n0, int lane) {
+  const int ra = lane >> 2, rb = ra + 8;
+  const bool va = ra < rows_valid, vb = rb < rows_valid;
+  const int img = rows_valid > 0 ? (int)gm / e.rows_per_img : 0;   // row counts stay below 2^31
+  const float* rv = e.rowvec ? e.rowvec + (long long)img * e.rowvec_ld : nullptr;
   const float scale = e.scale;
-  float sA = 0.f, qA = 0.f, sB = 0.f, qB = 0.f;
-  // all eight residual quads are requested before the first store: the output may alias the residual as far as
-  // the compiler knows, so loads left inside the store loop are serialised behind the stores (seen as one
-  // long-scoreboard stall per row in the attention kernel's profile)
-  float4 rr[8];
-  if (RES) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = r0 + 4 * i;
-      rr[i] = row < rows_valid ? __ldg(reinterpret_cast<const float4*>(e.residual + (gm0 + row) * e.ld_res + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    float2 ad = make_float2(0.f, 0.f);
+    if (e.bias) ad = __ldg(reinterpret_cast<const float2*>(e.bias + col));
+    if (rv) { const float2 t = __ldg(reinterpret_cast<const float2*>(rv + col)); ad.x += t.x; ad.y += t.y; }
+    float o0 = d[4 * j] + ad.x, o1 = d[4 * j + 1] + ad.y, o2 = d[4 * j + 2] + ad.x, o3 = d[4 * j + 3] + ad.y;
+    if (RES) {
+      if (va) { const float2 r = __ldg(reinterpret_cast<const float2*>(e.residual + (gm + ra) * e.ld_res + col)); o0 += r.x; o1 += r.y; }
+      if (vb) { const float2 r = __ldg(reinterpret_cast<const float2*>(e.residual + (gm + rb) * e.ld_res + col)); o2 += r.x; o3 += r.y; }
     }
-  }
+    o0 *= scale; o1 *= scale; o2 *= scale; o3 *= scale;
+    if (MODE == 1) { o0 = round_tf32(o0); o1 = round_tf32(o1); o2 = round_tf32(o2); o3 = round_tf32(o3); }
+    if (MODE == 2) {
+      uint16_t* oh = reinterpret_cast<uint16_t*>(e.out);
+      if (va) *reinterpret_cast<uint32_t*>(oh + (gm + ra) * e.ld_out + col) = pack_half2(o0, o1);
+      if (vb) *reinterpret_cast<uint32_t*>(oh + (gm + rb) * e.ld_out + col) = pack_half2(o2, o3);
+    } else {
+      if (va) *reinterpret_cast<float2*>(e.out + (gm + ra) * e.ld_out + col) = make_float2(o0, o1);
+      if (vb) *reinterpret_cast<float2*>(e.out + (gm + rb) * e.ld_out + col) = make_float2(o2, o3);
+    }
+    if (STATS) {
+      float s = (va ? o0 + o1 : 0.f) + (vb ? o2 + o3 : 0.f);
+      float q = (va ? fmaf(o0, o0, o1 * o1) : 0.f) + (vb ? fmaf(o2, o2, o3 * o3) : 0.f);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int row = r0 + 4 * i;
-    float4 o = lds128(tb + row * 128 + ((cq ^ (row & 7)) << 4));
-    if (row < rows_valid) {
-      const long long g = gm0 + row;
-      const bool second = two_img && i >= 4;                 // rows 16..31 of the block: the next image
-      const float4 ad = second ? addB : addA;
-      o.x += ad.x; o.y += ad.y; o.z += ad.z; o.w += ad.w;
-      if (RES) { o.x += rr[i].x; o.y += rr[i].y; o.z += rr[i].z; o.w += rr[i].w; }
-      o.x *= scale; o.y *= scale; o.z *= scale; o.w *= scale;
-      if (MODE == 1) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-      if (MODE == 2) *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(e.out) + g * e.ld_out + col) = make_uint2(pack_half2(o.x, o.y), pack_half2(o.z, o.w));
-      else *reinterpret_cast<float4*>(e.out + g * e.ld_out + col) = o;
-      if (STATS) {
-        const float s = (o.x + o.y) + (o.z + o.w), q2 = fmaf(o.x, o.x, o.y * o.y) + fmaf(o.z, o.z, o.w * o.w);
-        if (second) { sB += s; qB += q2; } else { sA += s; qA += q2; }
+      for (int m = 4; m <= 16; m <<= 1) { s += __shfl_xor_sync(0xffffffffu, s, m); q += __shfl_xor_sync(0xffffffffu, q, m); }
+      s += __shfl_xor_sync(0xffffffffu, s, 1); q += __shfl_xor_sync(0xffffffffu, q, 1);
+      if ((lane & ~2) == 0 && rows_valid > 0) {   // lanes 0 and 2: the two column quads of this 8-column group
+        double* qd = qstats + ((long long)img * (n_total >> 2) + (col >> 2)) * 2;
+        atomicAdd(qd, (double)s); atomicAdd(qd + 1, (double)q);
       }
     }
   }
-  __syncwarp();                                            // the scratch block is free for the next chunk
-  if (STATS) {
-    sA += __shfl_xor_sync(0xffffffffu, sA, 8); qA += __shfl_xor_sync(0xffffffffu, qA, 8);
-    sA += __shfl_xor_sync(0xffffffffu, sA, 16); qA += __shfl_xor_sync(0xffffffffu, qA, 16);
-    if (two_img) {
-      sB += __shfl_xor_sync(0xffffffffu, sB, 8); qB += __shfl_xor_sync(0xffffffffu, qB, 8);
-      sB += __shfl_xor_sync(0xffffffffu, sB, 16); qB += __shfl_xor_sync(0xffffffffu, qB, 16);
-    }
-    if (r0 == 0 && rows_valid > 0) {
-      double* qd = qstats + ((long long)img0 * (n_total >> 2) + (col >> 2)) * 2;
-      atomicAdd(qd, (double)sA); atomicAdd(qd + 1, (double)qA);
-      if (two_img && rows_valid > 16) { qd += (long long)(n_total >> 2) * 2; atomicAdd(qd, (double)sB); atomicAdd(qd + 1, (double)qB); }
-    }
-  }
 }
-__device__ __forceinline__ void row_chunk_t_dispatch(const uint32_t (&v)[32], uint8_t* tbuf, const Epilogue& e, double* qstats, int n_total,
-                                                     long long gm0, int rows_valid, int n0, int img0, int lane) {
+template <int BN>
+__device__ __forceinline__ void frag_rows_dispatch(const float (&d)[BN / 2], const Epilogue& e, double* qstats, int n_total,
+                                                   long long gm, int rows_valid, int n0, int lane) {
   const int mode = e.round_tf32;
   const bool has_res = e.residual != nullptr, stats = qstats != nullptr;
-#define B200_ROWT(R, M) do { if (stats) row_chunk_t<R, M, true>(v, tbuf, e, qstats, n_total, gm0, rows_valid, n0, img0, lane); \
-                             else row_chunk_t<R, M, false>(v, tbuf, e, qstats, n_total, gm0, rows_valid, n0, img0, lane); } while (0)
-  if (has_res) { if (mode == 0) B200_ROWT(true, 0); else if (mode == 1) B200_ROWT(true, 1); else B200_ROWT(true, 2); }
-  else { if (mode == 0) B200_ROWT(false, 0); else if (mode == 1) B200_ROWT(false, 1); else B200_ROWT(false, 2); }
-#undef B200_ROWT
+#define B200_ROWF(R, M) do { if (stats) frag_rows<BN, R, M, true>(d, e, qstats, n_total, gm, rows_valid, n0, lane); \
+                             else frag_rows<BN, R, M, false>(d, e, qstats, n_total, gm, rows_valid, n0, lane); } while (0)
+  if (has_res) { if (mode == 0) B200_ROWF(true, 0); else if (mode == 1) B200_ROWF(true, 1); else B200_ROWF(true, 2); }
+  else { if (mode == 0) B200_ROWF(false, 0); else if (mode == 1) B200_ROWF(false, 1); else B200_ROWF(false, 2); }
+#undef B200_ROWF
+}
+
+// Epilogue of one warp's 16-channel x 256-pixel slice of a swapped tile (D^T = W X^T: rows = output channels, columns =
+// pixels of ONE image).  Lane l holds channels c0 + l/4 and c0 + l/4 + 8 of pixel pairs 8j + 2(l%4); eight lanes cover 32
+// contiguous bytes of a pixel's channel vector.
+template <bool RES, int MODE, bool STATS>
+__device__ __forceinline__ void frag_swap(const float (&d)[128], const Epilogue& e, double* qstats, int n_total,
+                                          int c0, long long pix0, int img, int lane) {
+  const int ca = c0 + (lane >> 2), cb = ca + 8;
+  const float adda = (e.bias ? __ldg(e.bias + ca) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + ca) : 0.f);
+  const float addb = (e.bias ? __ldg(e.bias + cb) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + cb) : 0.f);
+  const float scale = e.scale;
+  float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const long long px = pix0 + 8 * j + 2 * (lane & 3);
+    float o[4] = {d[4 * j] + adda, d[4 * j + 1] + adda, d[4 * j + 2] + addb, d[4 * j + 3] + addb};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const long long pix = px + (i & 1);
+      const int ch = i < 2 ? ca : cb;
+      if (RES) o[i] += __ldg(e.residual + pix * e.ld_res + ch);
+      o[i] *= scale;
+      if (MODE == 1) o[i] = round_tf32(o[i]);
+      if (MODE == 2) {
+        uint16_t h;
+        asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(o[i]));
+        reinterpret_cast<uint16_t*>(e.out)[pix * e.ld_out + ch] = h;
+      } else e.out[pix * e.ld_out + ch] = o[i];
+    }
+    if (STATS) {
+      sa += o[0] + o[1]; qa = fmaf(o[0], o[0], fmaf(o[1], o[1], qa));
+      sb += o[2] + o[3]; qb = fmaf(o[2], o[2], fmaf(o[3], o[3], qb));
+    }
+  }
+  if (STATS) {
+#pragma unroll
+    for (int m = 1; m <= 8; m <<= 1) {   // pixel lanes (1, 2), then the four channels of a quad (4, 8)
+      sa += __shfl_xor_sync(0xffffffffu, sa, m); qa += __shfl_xor_sync(0xffffffffu, qa, m);
+      sb += __shfl_xor_sync(0xffffffffu, sb, m); qb += __shfl_xor_sync(0xffffffffu, qb, m);
+    }
+    if ((lane & 15) == 0) {
+      double* qd = qstats + ((long long)img * (n_total >> 2) + (ca >> 2)) * 2;
+      atomicAdd(qd, (double)sa); atomicAdd(qd + 1, (double)qa);
+      qd = qstats + ((long long)img * (n_total >> 2) + (cb >> 2)) * 2;
+      atomicAdd(qd, (double)sb); atomicAdd(qd + 1, (double)qb);
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------
 // Kernel
 // ---------------------------------------------------------------------------
-template <int BN, int STAGES>
-__global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  using L = SmemLayout<BN, STAGES>;
+// Consumer side of gemm_tc_kernel: one MMA warpgroup (g = 0, 1) owns accumulator rows 64g .. 64g + 63 of every tile.
+// A K step is released to the producer once the wgmma after it has been issued (wait_group 1), so the tensor core
+// always has the next step queued while the previous one's slot is handed back.
+template <int BN, bool F16>
+__device__ __forceinline__ void gemm_tc_consumer(const TcParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                                 uint64_t* wfull_bar, uint64_t* wempty_bar, int g, int wq, int lane) {
+  using L = SmemLayout<BN>;
+  const int kiters = (p.kchunks1 + p.kchunks2) * p.taps + p.kchunks3 + p.kchunks4;
+  const Epilogue& e = p.epi;
+  uint32_t stage = 0, phase = 0, ws = 0, wphase = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    float acc[BN / 2];
+    if (BN == 256 && p.halo) {
+      // halo form: A = the 16 KB weight slice (128 output channels), B = 256 pixel rows of a halo copy starting one filter
+      // row (W pixels) further in per dh; the slice's slot is released per tap, the copy's after its three taps
+      const uint32_t wring = smem_u32(smem + HALO_XS * HALO_X_BYTES);
+      int it = 0, pend_ws = -1, pend_x = -1;
+      for (int src = 0; src < 4; ++src) {
+        const int nch = src == 0 ? p.kchunks1 : src == 1 ? p.kchunks2 : src == 2 ? p.kchunks3 : p.kchunks4;
+        const int ncopies = src < 2 ? 3 * nch : nch, ntap = src < 2 ? 3 : 1;
+        for (int c = 0; c < ncopies; ++c) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sx = smem_u32(smem + stage * HALO_X_BYTES);
+          for (int dhi = 0; dhi < ntap; ++dhi, ++it) {
+            mbar_wait(&wfull_bar[ws], wphase);
+            const uint64_t adesc = make_smem_desc(wring + ws * A_STAGE_BYTES + g * (A_STAGE_BYTES / 2));
+            const uint64_t bdesc = make_smem_desc(sx + (src < 2 ? dhi * p.halo_dh_bytes : 0));
+            wgmma_kstep<BN, F16>(acc, adesc, bdesc, it);
+            wgmma_wait<1>();
+            if (lane == 0) {
+              if (pend_ws >= 0) mbar_arrive(&wempty_bar[pend_ws]);
+              if (pend_x >= 0) mbar_arrive(&empty_bar[pend_x]);
+            }
+            pend_ws = (int)ws; pend_x = dhi == ntap - 1 ? (int)stage : -1;
+            if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
+          }
+          if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
+        }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) {
+        if (pend_ws >= 0) mbar_arrive(&wempty_bar[pend_ws]);
+        if (pend_x >= 0) mbar_arrive(&empty_bar[pend_x]);
+      }
+    } else {
+      int pend = -1;
+      for (int it = 0; it < kiters; ++it) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
+        wgmma_kstep<BN, F16>(acc, make_smem_desc(sa + g * (A_STAGE_BYTES / 2)), make_smem_desc(sa + A_STAGE_BYTES), it);
+        wgmma_wait<1>();
+        if (lane == 0 && pend >= 0) mbar_arrive(&empty_bar[pend]);
+        pend = (int)stage;
+        if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (lane == 0 && pend >= 0) mbar_arrive(&empty_bar[pend]);
+    }
+
+    // ---- epilogue: this warp's 16 accumulator rows ----
+    const int rw = g * 64 + wq * 16;                       // first tile row of this warp
+    if constexpr (BN == 256) {
+      if (p.swap) {
+        // swapped operands (128-channel layers, 1x1 convolutions, the head): rows = output channels, columns = 256 pixels
+        const int c0 = (int)(tile % p.tiles_n) * 128 + rw;
+        const int pix0 = (tile / p.tiles_n) * 256;
+        const int img = pix0 / e.rows_per_img;     // rows_per_img % 256 == 0: one image per tile
+        if (e.out_nchw) {
+          // Network head (ncsnpp.py:374-380): the 128-row weight tile is zero-padded above the n_valid image channels;
+          // (acc + bias) / sigma[img] is written as NCHW
+          const float dv = e.per_img_div ? __ldg(e.per_img_div + img * e.div_stride) : 1.f;
+          const int hw = e.rows_per_img, pix_in_img = (int)(pix0 - (long long)img * hw);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int co = c0 + (lane >> 2) + 8 * h;
+            if (co < e.n_valid) {
+              const float add = e.bias ? __ldg(e.bias + co) : 0.f;
+              float* dst = e.out + ((long long)img * e.n_valid + co) * hw + pix_in_img + 2 * (lane & 3);
+#pragma unroll
+              for (int j = 0; j < 32; ++j)
+                *reinterpret_cast<float2*>(dst + 8 * j) = make_float2((acc[4 * j + 2 * h] + add) / dv, (acc[4 * j + 2 * h + 1] + add) / dv);
+            }
+          }
+        } else {
+          const int mode = e.round_tf32;
+          const bool has_res = e.residual != nullptr, stats = p.qstats != nullptr;
+#define B200_SWAPF(R, M) do { if (stats) frag_swap<R, M, true>(acc, e, p.qstats, p.N_total, c0, pix0, img, lane); \
+                              else frag_swap<R, M, false>(acc, e, p.qstats, p.N_total, c0, pix0, img, lane); } while (0)
+          if (has_res) { if (mode == 0) B200_SWAPF(true, 0); else if (mode == 1) B200_SWAPF(true, 1); else B200_SWAPF(true, 2); }
+          else { if (mode == 0) B200_SWAPF(false, 0); else if (mode == 1) B200_SWAPF(false, 1); else B200_SWAPF(false, 2); }
+#undef B200_SWAPF
+        }
+        continue;
+      }
+    }
+    const int nt = (int)(tile % p.tiles_n);
+    const int mg = tile / p.tiles_n;
+    const int b = (int)(mg / p.tiles_m_per_batch);
+    const int mt = (int)(mg % p.tiles_m_per_batch);
+    const int row0 = mt * BM + rw;
+    const int rows_valid = min(16, max(0, p.M_per_batch - row0));
+    frag_rows_dispatch<BN>(acc, e, p.qstats, p.N_total, (long long)b * p.M_per_batch + row0, rows_valid, nt * BN, lane);
+  }
+}
+
+template <int BN>
+__global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__ TcParams p) {
+  using L = SmemLayout<BN>;
+  constexpr int STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  uint64_t* wfull_bar = tmem_empty + 3;          // halo form: the weight-slice ring has its own barriers
+  uint64_t* wfull_bar = empty_bar + STAGES;      // halo form: the weight-slice ring has its own barriers
   uint64_t* wempty_bar = wfull_bar + HALO_WS;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp index provably warp-uniform
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < HALO_WS; ++s) { mbar_init(&wfull_bar[s], 1); mbar_init(&wempty_bar[s], 1); }
-    // one arrival per epilogue warp (384 threads: two warps per TMEM lane quarter)
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], (blockDim.x >> 5) - 4); }
+    // empty slots: one arrival per MMA warp (8)
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int s = 0; s < HALO_WS; ++s) { mbar_init(&wfull_bar[s], 1); mbar_init(&wempty_bar[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * BN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait(); pdl_trigger();   // barriers and TMEM are set up; nothing above touched global memory (common.cuh)
+  pdl_wait(); pdl_trigger();   // barriers are set up; nothing above touched global memory (common.cuh)
 
-  const int kiters = (p.kchunks1 + p.kchunks2) * p.taps + p.kchunks3 + p.kchunks4;
   const int HW = p.H * p.W;
   const int bke = p.bke;
 
-  if (warp == 0) {
+  if (warp < 4) {
+    regs_producer();
+    if (warp != 0) return;
     // ======================= TMA producer (whole warp; one elected lane issues, see elect_one) =======================
     const bool issue = elect_one();
     uint32_t stage = 0, phase = 0;
@@ -485,13 +424,13 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
       // followed by the three 16 KB weight slices of its filter column
       uint32_t ws = 0, wphase = 0;
       uint8_t* const wring = smem + HALO_XS * HALO_X_BYTES;
-      for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int nt = (int)(tile % p.tiles_n);
-        const long long p0 = (tile / p.tiles_n) * 256;
+        const int p0 = (tile / p.tiles_n) * 256;
         const int img0 = (int)(p0 / HW), h0 = (int)(p0 % HW) / p.W;
         const int wrow0 = nt * 128;
         if (issue && p.halo_prefetch && tile + gridDim.x < p.total_tiles && (tile + gridDim.x) / p.tiles_n != tile / p.tiles_n) {
-          const long long q0 = ((tile + gridDim.x) / p.tiles_n) * 256;                 // next tile of this CTA: its pixels, every chunk
+          const int q0 = ((tile + gridDim.x) / p.tiles_n) * 256;                 // next tile of this CTA: its pixels, every chunk
           const int qi = (int)(q0 / HW), qh = (int)(q0 % HW) / p.W;
           for (int kc = 0; kc < p.kchunks1; ++kc) tma_prefetch_4d(&p.tmH1, kc * bke, 0, qh - 1, qi);
           for (int kc = 0; kc < p.kchunks2; ++kc) tma_prefetch_4d(&p.tmH2, kc * bke, 0, qh - 1, qi);
@@ -541,14 +480,14 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
         }
       }
     } else
-    for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const int nt = (int)(tile % p.tiles_n);
-      const long long mg = tile / p.tiles_n;
+      const int mg = tile / p.tiles_n;
       const int b = (int)(mg / p.tiles_m_per_batch);
       const int mt = (int)(mg % p.tiles_m_per_batch);
       int img0 = 0, h0 = 0, w0 = 0;
       if (p.conv) {
-        const long long p0 = (long long)mt * BM;
+        const int p0 = (long long)mt * BM;
         img0 = (int)(p0 / HW);
         const int rem = (int)(p0 % HW);
         h0 = rem / p.W; w0 = rem % p.W;
@@ -557,9 +496,9 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
       const int wrow0 = b * p.w_batch_rows + nt * (p.swap ? 128 : BN);
       int img1 = 0, h1 = 0, w1 = 0;                     // swap mode: second 128-pixel box of the 256-pixel tile
       if (p.swap) {
-        const long long p0 = (long long)mt * 256;
+        const int p0 = (long long)mt * 256;
         img0 = (int)(p0 / HW); h0 = (int)(p0 % HW) / p.W; w0 = (int)(p0 % HW) % p.W;
-        const long long p1 = p0 + 128;
+        const int p1 = p0 + 128;
         img1 = (int)(p1 / HW); h1 = (int)(p1 % HW) / p.W; w1 = (int)(p1 % HW) % p.W;
       }
       // sources 0,1: the (two-source) filter input, all taps; sources 2,3: the extra 1x1 phase (centre tap, own weights)
@@ -571,8 +510,7 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
         const int wcol0 = src == 1 ? p.C1 : src == 3 ? p.C3 : 0;
         const int ntaps = src < 2 ? p.taps : 1;
         // K order.  Default: filter tap, then channel chunk - consecutive loads sweep the channel vector of the same shifted
-        // pixels (contiguous 128-byte segments of every pixel row; measured ~30 % faster than the other order in the
-        // CTA-pair kernel, profiles/r02_f3_*).  Shapes that have a halo form (p.chunk_major) walk K the way that form must -
+        // pixels (contiguous 128-byte segments of every pixel row).  Shapes that have a halo form (p.chunk_major) walk K the way that form must -
         // channel chunk, filter column, filter row - so that halo on / off add the same products in the same order and
         // are bit-identical (the nine-load loop of such a shape only runs in A/B checks).
         const int nouter = p.chunk_major ? nch : ntaps, ninner = p.chunk_major ? ntaps : nch;
@@ -587,7 +525,7 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
             if (issue) {
               mbar_expect_tx(&full_bar[stage], L::STAGE_BYTES);
               if (p.swap) {
-                // first 16 KiB: 128 output channels x 32 k of W (UMMA A); next 32 KiB: 256 pixels x 32 k (UMMA B)
+                // first 16 KiB: 128 output channels x 32 k of W (MMA A); next 32 KiB: 256 pixels x 32 k (MMA B)
                 tma_load_2d(tmW, sa, &full_bar[stage], wcol0 + kc * bke, wrow0 + tap * p.N_total);
                 tma_load_4d(tmA, sb, &full_bar[stage], kc * bke, w0 + dw, h0 + dh, img0);
                 tma_load_4d(tmA, sb + A_STAGE_BYTES, &full_bar[stage], kc * bke, w1 + dw, h1 + dh, img1);
@@ -602,202 +540,15 @@ __global__ void __maxnreg__(160) gemm_tc_kernel(const __grid_constant__ TcParams
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer (whole warp; one elected lane issues) =======================
-    const bool issue = elect_one();
-    const bool f16 = p.f16 != 0;
-    const uint32_t idesc = f16 ? make_idesc_f16<BN>() : make_idesc<BN>();
-    uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-    if (BN == 256 && p.halo) {
-      // halo form: A = the 16 KB weight slice (128 output channels), B = 256 pixel rows of a halo copy starting one filter
-      // row (W pixels) further in per dh; the slice's slot is released per tap, the copy's after its three taps
-      uint32_t ws = 0, wphase = 0;
-      const uint32_t wring = smem_u32(smem + HALO_XS * HALO_X_BYTES);
-      for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        int it = 0;
-        for (int src = 0; src < 4; ++src) {
-          const int nch = src == 0 ? p.kchunks1 : src == 1 ? p.kchunks2 : src == 2 ? p.kchunks3 : p.kchunks4;
-          const int ncopies = src < 2 ? 3 * nch : nch, ntap = src < 2 ? 3 : 1;
-          for (int c = 0; c < ncopies; ++c) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t sx = smem_u32(smem + stage * HALO_X_BYTES);
-            for (int dhi = 0; dhi < ntap; ++dhi, ++it) {
-              mbar_wait(&wfull_bar[ws], wphase);
-              tc_fence_after();
-              const uint64_t adesc = make_smem_desc(wring + ws * A_STAGE_BYTES);
-              const uint64_t bdesc = make_smem_desc(sx + (src < 2 ? dhi * p.halo_dh_bytes : 0));
-              if (issue) {
-                if (f16) umma_kstep<true>(d_tmem, adesc, bdesc, idesc, it);
-                else umma_kstep<false>(d_tmem, adesc, bdesc, idesc, it);
-                umma_commit(&wempty_bar[ws]);
-              }
-              if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
-            }
-            if (issue) umma_commit(&empty_bar[stage]);
-            if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (issue) umma_commit(&tmem_full[acc]);
-        acc ^= 1; if (acc == 0) acc_phase ^= 1;
-      }
-    } else
-    for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int it = 0; it < kiters; ++it) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-        const uint64_t adesc = make_smem_desc(sa);
-        const uint64_t bdesc = make_smem_desc(sa + A_STAGE_BYTES);
-        if (issue) {
-          if (f16) umma_kstep<true>(d_tmem, adesc, bdesc, idesc, it);
-          else umma_kstep<false>(d_tmem, adesc, bdesc, idesc, it);
-          umma_commit(&empty_bar[stage]);
-        }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (issue) umma_commit(&tmem_full[acc]);
-      acc ^= 1; if (acc == 0) acc_phase ^= 1;
-    }
-  } else if (warp >= 4) {
-    // ======================= epilogue (direct stores) =======================
-    // Eight warps: warp w may touch TMEM lanes 32*(w%4).., so warps 4..7 and 8..11 pair up on each lane quarter
-    // and split the tile's columns — twice the loads/stores in flight for the output-bound (small-K) launches.
-    const int q = (warp - 4) & 3;              // TMEM lane quarter owned by this warp
-    const int half = (warp - 4) >> 2;          // which half of the tile's columns
-    const int r = q * 32 + lane;               // row of the tile held by this thread
-    const Epilogue& e = p.epi;
-    uint32_t acc = 0, acc_phase = 0;
-    if (p.swap) {
-      // Swapped operands (D^T = W X^T, 128-channel layers): TMEM lane = output channel, column = pixel.  A warp's
-      // 32 lanes are 32 consecutive channels of one pixel, so every scalar load/store instruction below touches
-      // exactly one 128-byte line of the NHWC tensor (fully coalesced), and the M=128 x N=256 instruction keeps the
-      // single issuing thread ahead of the tensor pipe (N=128 instructions retire in 64 cycles, faster than one
-      // thread can issue them).
-      if constexpr (BN == 256) {
-        for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-          const int co = (int)(tile % p.tiles_n) * 128 + r;
-          const long long row_base = (tile / p.tiles_n) * 256;
-          const int img = (int)(row_base / e.rows_per_img);          // rows_per_img % 256 == 0: one image per tile
-          const float add = (e.bias ? __ldg(e.bias + co) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + co) : 0.f);
-          float ssum = 0.f, ssq = 0.f;
-          if (e.out_nchw) {
-            // Network head (ncsnpp.py:374-380): the 128-row weight tile is zero-padded above the n_valid image
-            // channels, so only lanes < n_valid of lane quarter 0 hold results: (acc + bias) / sigma[img], written
-            // as NCHW with 128-bit stores along the pixel axis.  The other warps just release the accumulator.
-            mbar_wait(&tmem_full[acc], acc_phase);
-            tc_fence_after();
-            if (q == 0) {
-              const float dv = e.per_img_div ? __ldg(e.per_img_div + img * e.div_stride) : 1.f;
-              const int hw = e.rows_per_img, pix_in_img = (int)(row_base - (long long)img * hw);
-#pragma unroll 1
-              for (int j = half * 4; j < half * 4 + 4; ++j) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + acc * BN + j * 32, v);
-                if (lane < e.n_valid) {
-                  float* dst = e.out + ((long long)img * e.n_valid + lane) * hw + pix_in_img + j * 32;
-#pragma unroll
-                  for (int i = 0; i < 32; i += 4)
-                    *reinterpret_cast<float4*>(dst + i) = make_float4((__uint_as_float(v[i]) + add) / dv, (__uint_as_float(v[i + 1]) + add) / dv,
-                                                                      (__uint_as_float(v[i + 2]) + add) / dv, (__uint_as_float(v[i + 3]) + add) / dv);
-                }
-              }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-            acc ^= 1; if (acc == 0) acc_phase ^= 1;
-            continue;
-          }
-          if (e.residual) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j)   // this lane's share of the warp's 128 residual lines (one per pixel)
-              prefetch_l2(e.residual + (row_base + half * 128 + j * 32 + lane) * e.ld_res + (int)(tile % p.tiles_n) * 128 + q * 32);
-          }
-          mbar_wait(&tmem_full[acc], acc_phase);
-          tc_fence_after();
-          const int mode = e.round_tf32;
-          const bool has_res = e.residual != nullptr;
-#pragma unroll 1
-          for (int j = half * 4; j < half * 4 + 4; ++j) {
-            uint32_t v[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + j * 32, v);
-            const long long pix0 = row_base + j * 32;
-            const float* res = has_res ? e.residual + pix0 * e.ld_res + co : nullptr;
-            // element offset of (pix0, co); fp16 outputs count halves from the same base pointer
-            float* dst = mode == 2 ? reinterpret_cast<float*>(reinterpret_cast<uint16_t*>(e.out) + pix0 * e.ld_out + co)
-                                   : e.out + pix0 * e.ld_out + co;
-            if (has_res) {
-              if (mode == 0) swap_chunk<true, 0>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-              else if (mode == 1) swap_chunk<true, 1>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-              else swap_chunk<true, 2>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-            } else {
-              if (mode == 0) swap_chunk<false, 0>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-              else if (mode == 1) swap_chunk<false, 1>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-              else swap_chunk<false, 2>(v, add, e.scale, dst, res, e.ld_out, e.ld_res, ssum, ssq);
-            }
-          }
-          if (p.qstats) {
-            ssum += __shfl_xor_sync(0xffffffffu, ssum, 1); ssq += __shfl_xor_sync(0xffffffffu, ssq, 1);
-            ssum += __shfl_xor_sync(0xffffffffu, ssum, 2); ssq += __shfl_xor_sync(0xffffffffu, ssq, 2);
-            if ((lane & 3) == 0) {
-              double* qd = p.qstats + ((long long)img * (p.N_total >> 2) + (co >> 2)) * 2;
-              atomicAdd(qd, (double)ssum); atomicAdd(qd + 1, (double)ssq);
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-          acc ^= 1; if (acc == 0) acc_phase ^= 1;
-        }
-      }
-    } else
-    for (long long tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int nt = (int)(tile % p.tiles_n);
-      const long long mg = tile / p.tiles_n;
-      const int b = (int)(mg / p.tiles_m_per_batch);
-      const int mt = (int)(mg % p.tiles_m_per_batch);
-      const int row0 = mt * BM + q * 32;                                   // first row of this warp's 32-row blocks
-      const int rows_valid = min(32, max(0, p.M_per_batch - row0));
-      const long long gm0 = (long long)b * p.M_per_batch + row0;
-      const int img0 = rows_valid > 0 ? (int)(gm0 / e.rows_per_img) : 0;
-      if (e.residual && lane < rows_valid) {   // residual rows -> L2 while the accumulator is still being produced
-#pragma unroll
-        for (int i = 0; i < BN / 2; i += 32) prefetch_l2(e.residual + (gm0 + lane) * e.ld_res + nt * BN + half * (BN / 2) + i);
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int j = half * (BN / 64); j < (half + 1) * (BN / 64); ++j) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN + j * 32, v);
-        row_chunk_t_dispatch(v, smem + L::TRN_OFFSET + (warp - 4) * 4096, e, p.qstats, p.N_total, gm0, rows_valid,
-                               nt * BN + j * 32, img0, lane);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      acc ^= 1; if (acc == 0) acc_phase ^= 1;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * BN) : "memory");
+  } else {
+    regs_consumer();
+    const int g = (warp >> 2) - 1, wq = warp & 3;   // MMA warpgroup and warp within it
+    if (p.f16) gemm_tc_consumer<BN, true>(p, smem, full_bar, empty_bar, wfull_bar, wempty_bar, g, wq, lane);
+    else gemm_tc_consumer<BN, false>(p, smem, full_bar, empty_bar, wfull_bar, wempty_bar, g, wq, lane);
   }
 }
 
-#include "gemm_tc2.cuh"
 #include "attn_tc.cuh"
-#include "gemm_tcg.cuh"
 
 // ---------------------------------------------------------------------------
 // Host side: tensor maps, plan, launch
@@ -834,7 +585,7 @@ int encode_map(CUtensorMap* tm, const float* base, int rank, const uint64_t* dim
 
 int num_sms() {
   static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
   return n;
 }
 
@@ -843,7 +594,6 @@ int num_sms() {
 struct TcGemmPlan {
   TcParams prm;
   int bn;
-  bool two_cta;
 };
 
 static int tc_configure();
@@ -902,12 +652,10 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
   const uint64_t es = f16 ? 2 : 4;           // operand element size
   p.bke = bke;
   {
-    // Form selection (each choice measured against the alternatives in round 1, DESIGN.md section 4.1):
+    // Form selection:
     //  * swapped operands (D^T = W X^T: 128 output channels x 256 pixels per tile) for 128-channel outputs, whose
     //    M=128,N=128 MMAs are issue-bound, and for 1x1 convolutions (output-bound launches: the swapped form's
-    //    epilogue is perfectly coalesced, 12-20 % faster, profiles/r01_c11_exp.log); the NCHW head exists only in this form;
-    //  * CTA pairs (cta_group::2) for 256-column tiles when the launch has at least one 256-row pair per cluster
-    //    slot (small launches fill the SMs better with single-CTA tiles); `no_pair` in the descriptor opts out;
+    //    epilogue writes whole channel vectors of a pixel); the NCHW head exists only in this form;
     //  * launches too small to give every SM a 256-column tile are cut into 128-column tiles: twice the CTAs at work.
     const long long Mtot = (long long)d.nimg * d.H * d.W;
     // (image rows wider than 128 pixels - the 256..1024-pixel families - are cut into 128-pixel boxes like any other: the
@@ -921,9 +669,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     const int tmb = d.conv ? 1 : (d.M_per_batch + BM - 1) / BM;
     const long long m_tiles = d.conv ? (Mtot + BM - 1) / BM : (long long)d.nbatch * tmb;
     const long long n_tiles = d.N_total % 256 == 0 ? d.N_total / 256 : d.N_total / 128;
-    pl->two_cta = !d.no_pair && !p.swap && d.N_total % 256 == 0 &&
-                  (d.conv || d.nbatch == 1 || tmb % 2 == 0) && (m_tiles / 2) * n_tiles >= num_sms() / 2;
-    if (!pl->two_cta && !p.swap && pl->bn == 256 && m_tiles * n_tiles <= num_sms() / 2) pl->bn = 128;
+    if (!p.swap && pl->bn == 256 && m_tiles * n_tiles <= num_sms() / 2) pl->bn = 128;
   }
   p.kchunks1 = d.C1 / bke; p.kchunks2 = d.a2 ? d.C2 / bke : 0; p.C1 = d.C1;
   p.N_total = d.N_total; p.tiles_n = p.swap ? d.N_total / 128 : d.N_total / pl->bn;
@@ -968,24 +714,23 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
   p.tmA3 = p.tmA1; p.tmA4 = p.tmA1;
   p.tmH1 = p.tmA1; p.tmH2 = p.tmA1;
   {
-    // Halo form (DESIGN.md section 4.13): 'same'-padded stride-1 3x3 filters on 16- or 32-pixel-wide images, where the CTA's tile
-    // (256 pixels swapped, 128 pixels per CTA of a pair) is whole rows of ONE image: 3 loads of (rows + 2) x W pixels per
+    // Halo form: 'same'-padded stride-1 3x3 filters on 16- or 32-pixel-wide images, where the CTA's tile
+    // (256 pixels, swapped form) is whole rows of ONE image: 3 loads of (rows + 2) x W pixels per
     // channel chunk instead of 9 loads of rows x W - the plain form is bound by the L2 -> SM fill rate, not the tensor pipe.
     const int tile_px = p.swap ? 256 : BM;
-    const bool halo = (d.no_halo & 3) != 1 && d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && (p.swap || (pl->two_cta && (d.no_halo & 3) == 2)) &&
+    const bool halo = (d.no_halo & 3) != 1 && d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && p.swap &&
                       (d.W == 16 || d.W == 32) && (d.H * d.W) % tile_px == 0 && (d.Hin == 0 || d.Hin == d.H) && (d.Win == 0 || d.Win == d.W);
     // swapped-form shapes that have a halo form keep its K order when it is switched off (bit-identical A/B).  `no_halo & 8`
-    // asks the same of the single-CTA row-major kernel for shapes the CTA-pair kernel would run in halo form: a small-batch
-    // plan then adds the same products in the same order as the pair plan of a large batch (plan-agreement tests; the
-    // chunk-major nine-load loop is ~30 % slower, so nothing else sets it)
+    // asks the same of row-major launches of such shapes, so that plans of different batch sizes add the same products in
+    // the same order (plan-agreement tests)
     const bool halo_shape = d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && (d.W == 16 || d.W == 32) && (d.H * d.W) % tile_px == 0 &&
                             (d.Hin == 0 || d.Hin == d.H) && (d.Win == 0 || d.Win == d.W);
-    p.chunk_major = (halo_shape && (p.swap || ((d.no_halo & 8) && !pl->two_cta))) ? 1 : 0;
+    p.chunk_major = (halo_shape && (p.swap || (d.no_halo & 8))) ? 1 : 0;
     if (halo) {
       const int rows = tile_px / d.W;
       p.halo = 1; p.halo_dh_bytes = d.W * 128; p.halo_copy_bytes = (rows + 2) * d.W * 128;
       p.halo_prefetch = (d.no_halo & 4) ? 1 : 0;
-      B200_REQUIRE(p.halo_copy_bytes <= (p.swap ? HALO_X_BYTES : HALO2_X_BYTES), "gemm_tc: halo copy of %d bytes does not fit its slot", p.halo_copy_bytes);
+      B200_REQUIRE(p.halo_copy_bytes <= HALO_X_BYTES, "gemm_tc: halo copy of %d bytes does not fit its slot", p.halo_copy_bytes);
       uint32_t box[4] = {(uint32_t)bke, (uint32_t)d.W, (uint32_t)(rows + 2), 1};
       for (int s = 0; s < 2; ++s) {
         const float* base = s ? d.a2 : d.a1;
@@ -1019,7 +764,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
   {
     uint64_t dims[2] = {(uint64_t)d.K_total, (uint64_t)d.w_rows};
     uint64_t str[1] = {(uint64_t)(d.w_ld ? d.w_ld : d.K_total) * es};
-    uint32_t box[2] = {(uint32_t)bke, (uint32_t)(pl->two_cta ? pl->bn / 2 : (p.swap ? 128 : pl->bn))};
+    uint32_t box[2] = {(uint32_t)bke, (uint32_t)(p.swap ? 128 : pl->bn)};
     rc = encode_map(&p.tmW, d.w, 2, dims, str, box, nullptr, f16);
     if (rc) { delete pl; return rc; }
     p.tmW2 = p.tmW;
@@ -1038,7 +783,6 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
 
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 const char* tc_gemm_form(const TcGemmPlan* p) {
-  if (p->two_cta) return p->prm.halo ? "pair256-halo" : "pair256";
   if (p->prm.swap) return p->prm.halo ? "swap-halo" : "swap";
   return p->bn == 256 ? "single256" : "single128";
 }
@@ -1099,112 +843,29 @@ int tc_attn_launch(const TcAttnPlan* pl, cudaStream_t st) {
   return 0;
 }
 
-// ---- convolution with GroupNorm (+SiLU) applied on load (gemm_tcg.cuh) ----
-struct TcgPlan { TcgParams prm; };
-
-bool tcg_supported(const TcgDesc& d, const char** why) {
-  static const char* w;
-  auto fail = [&](const char* m) { w = m; if (why) *why = w; return false; };
-  if (d.W != 16 && d.W != 32) return fail("image width must be 16 or 32");
-  if (d.H <= 0 || (d.H * d.W) % 128 || d.H % (128 / d.W)) return fail("image rows do not tile 128 pixels");
-  if (d.N_total % 256) return fail("C_out must be a multiple of 256");
-  if (d.C1 <= 0 || d.C1 % 64 || d.C2 % 64 || d.C3 % 64 || d.C4 % 64) return fail("channel counts must be multiples of 64");
-  if ((d.a2 == nullptr) != (d.C2 == 0) || (d.a3 == nullptr) != (d.C3 == 0) || (d.a4 == nullptr) != (d.C4 == 0)) return fail("source / channel-count mismatch");
-  if (d.a4 && !d.a3) return fail("second extra source without the first");
-  if (d.a3 && !d.w2) return fail("extra 1x1 phase without weights");
-  if ((d.gn_scale == nullptr) != (d.gn_shift == nullptr)) return fail("GroupNorm scale and shift come together");
-  if (d.epi.out_nchw || d.epi.per_img_div) return fail("plain NHWC epilogue only");
-  if (d.epi.ld_out % 4 || (d.epi.residual && d.epi.ld_res % 4)) return fail("output pitch must be a multiple of 4 elements");
-  if (d.epi.round_tf32 == 2 && d.epi.ld_out % 8) return fail("fp16 output pitch must be a multiple of 8 elements");
-  if (d.epi.rows_per_img != d.H * d.W) return fail("rows_per_img must be H*W");
-  return true;
-}
-
-int tcg_plan_create(const TcgDesc& d, TcgPlan** out) {
-  const char* why = nullptr;
-  B200_REQUIRE(tcg_supported(d, &why), "gemm_tcg: unsupported shape: %s", why ? why : "?");
-  B200_REQUIRE(d.a1 && d.w && d.nimg > 0, "gemm_tcg: null argument");
-  if (int r = tc_configure()) return r;
-  TcgPlan* pl = new TcgPlan();
-  TcgParams& p = pl->prm;
-  memset(&p, 0, sizeof(p));
-  p.src[0] = d.a1; p.srcC[0] = d.C1; p.srcF16[0] = d.a1_f16; p.kch[0] = d.C1 / 64;
-  p.src[1] = d.a2; p.srcC[1] = d.C2; p.srcF16[1] = d.a2_f16; p.kch[1] = d.a2 ? d.C2 / 64 : 0;
-  p.src[2] = d.a3; p.srcC[2] = d.C3; p.srcF16[2] = d.a3_f16; p.kch[2] = d.a3 ? d.C3 / 64 : 0;
-  p.src[3] = d.a4; p.srcC[3] = d.C4; p.srcF16[3] = d.a4_f16; p.kch[3] = d.a4 ? d.C4 / 64 : 0;
-  for (int s = 0; s < 4; ++s)
-    if (p.src[s] && (reinterpret_cast<uintptr_t>(p.src[s]) & 15)) { delete pl; B200_REQUIRE(false, "gemm_tcg: source %d not 16-byte aligned", s); }
-  p.scale = d.gn_scale; p.shift = d.gn_shift; p.Cgn = d.C1 + d.C2; p.act = d.act;
-  p.H = d.H; p.W = d.W; p.R = 128 / d.W;
-  p.N_total = d.N_total; p.tiles_n = d.N_total / 256;
-  p.tiles_m = (long long)d.nimg * d.H * d.W / 128;
-  p.qstats = d.qstats; p.epi = d.epi;
-  {
-    const uint64_t K = (uint64_t)d.C1 + d.C2;
-    uint64_t dims[2] = {K, (uint64_t)9 * d.N_total};
-    uint64_t str[1] = {K * 2};
-    uint32_t box[2] = {64, 128};
-    int rc = encode_map(&p.tmW, d.w, 2, dims, str, box, nullptr, true);
-    p.tmW2 = p.tmW;
-    if (!rc && d.a3) {
-      const uint64_t K3 = (uint64_t)d.C3 + d.C4;
-      uint64_t dims2[2] = {K3, (uint64_t)d.N_total};
-      uint64_t str2[1] = {K3 * 2};
-      rc = encode_map(&p.tmW2, d.w2, 2, dims2, str2, box, nullptr, true);
-    }
-    if (rc) { delete pl; return rc; }
-  }
-  *out = pl;
-  return 0;
-}
-void tcg_plan_destroy(TcgPlan* p) { delete p; }
-void tcg_set_rowvec_ld(TcgPlan* p, long long ld) { p->prm.epi.rowvec_ld = ld; }
-int tcg_launch(const TcgPlan* pl, cudaStream_t st) {
-  const TcgParams& q = pl->prm;
-  const long long pairs = ((q.tiles_m + 1) / 2) * q.tiles_n;
-  if (pairs == 0) return 0;
-  const int grid = (int)std::min<long long>(2 * pairs, (long long)(num_sms() & ~1));
-  if (q.W == 32) launch_kernel(conv_gn2_kernel<true>, dim3(grid), dim3(TG_THREADS), SmemG::TOTAL, st, q);
-  else launch_kernel(conv_gn2_kernel<false>, dim3(grid), dim3(TG_THREADS), SmemG::TOTAL, st, q);
-  B200_CHECK_LAUNCH();
-  return 0;
-}
-
 // Opt in to the large dynamic shared-memory carve-out once, outside any stream capture.
 static int tc_configure() {
   static bool configured = false;
   if (configured) return 0;
-  B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<256, 4>::TOTAL));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<128, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<128, 6>::TOTAL));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<256, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem2<256, 6>::TOTAL));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<256>::TOTAL));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemLayout<128>::TOTAL));
   B200_CHECK_CUDA(cudaFuncSetAttribute(attn_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<false>::TOTAL));
   B200_CHECK_CUDA(cudaFuncSetAttribute(attn_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AttnSmem<true>::TOTAL));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(conv_gn2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemG::TOTAL));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(conv_gn2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemG::TOTAL));
   configured = true;
   return 0;
 }
 
-template <int BN, int STAGES>
+template <int BN>
 static int launch_impl(const TcGemmPlan* pl, cudaStream_t st) {
-  using L = SmemLayout<BN, STAGES>;
   const int grid = (int)std::min<long long>(pl->prm.total_tiles, num_sms());
-  launch_kernel(gemm_tc_kernel<BN, STAGES>, dim3(grid), dim3(384), L::TOTAL, st, pl->prm);
+  launch_kernel(gemm_tc_kernel<BN>, dim3(grid), dim3(384), SmemLayout<BN>::TOTAL, st, pl->prm);
   B200_CHECK_LAUNCH();
   return 0;
 }
 
 int tc_gemm_launch(const TcGemmPlan* pl, cudaStream_t st) {
   if (pl->prm.total_tiles == 0) return 0;
-  if (pl->two_cta) {
-    const TcParams& q = pl->prm;
-    const long long pairs = (((long long)q.nbatch * q.tiles_m_per_batch + 1) / 2) * q.tiles_n;
-    const int grid = (int)std::min<long long>(2 * pairs, (long long)(num_sms() & ~1));
-    launch_kernel(gemm_tc2_kernel<256, 6>, dim3(grid), dim3(384), Smem2<256, 6>::TOTAL, st, pl->prm);
-    B200_CHECK_LAUNCH();
-    return 0;
-  }
-  return pl->bn == 256 ? launch_impl<256, 4>(pl, st) : launch_impl<128, 6>(pl, st);
+  return pl->bn == 256 ? launch_impl<256>(pl, st) : launch_impl<128>(pl, st);
 }
 
 }  // namespace b200

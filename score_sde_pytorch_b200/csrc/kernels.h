@@ -77,7 +77,7 @@ int launch_conv_simt(const SimtConv& p, cudaStream_t st);
 bool conv_lowc_supported(const SimtConv& p);
 int launch_conv_lowc(const SimtConv& p, cudaStream_t st);
 
-// ---- gemm_tc.cu : tcgen05 / TMEM / TMA implicit GEMM (TF32 operands) -------
+// ---- gemm_tc.cu : wgmma / TMA implicit GEMM (TF32 or fp16 operands) --------
 struct TcGemmPlan;   // opaque, owns the encoded tensor maps
 struct TcGemmDesc {
   // A: NHWC activations, values already on the TF32 grid.
@@ -99,10 +99,9 @@ struct TcGemmDesc {
   // optional extra 1x1 phase accumulated into the same tile (a resblock's skip projection fused into its second
   // 3x3 convolution): out += [a3 | a4] w2^T, w2 = [N_total][C3 + C4]; same spatial size as the output, stride 1
   const float* a3; int C3; const float* a4; int C4; const float* w2;
-  int f16;                  // 1: a1..a4, w, w2 hold fp16 elements (tcgen05 kind::f16, 64-channel K steps); pitches stay in elements
-  int no_pair;              // 1 = never use the two-CTA (cta_group::2) kernel for this launch
+  int f16;                  // 1: a1..a4, w, w2 hold fp16 elements (wgmma .f16, 64-channel K steps); pitches stay in elements
   int no_halo;              // halo form of the 3x3 mainloop (three W-shifted halo copies per channel chunk instead of nine shifted
-                            // tiles): 0 = in the swapped form only (the measured winner), 1 = never, 2 = CTA pairs as well;
+                            // tiles): 0 or 2 = in the swapped form, 1 = never;
                             // + 4 = with an L2 prefetch (UTMAPF) of the next tile's halo boxes (A/B: measured 2 % slower);
                             // + 8 = single-CTA row-major launches of shapes the pair kernel runs in halo form walk K in that form's order
   double* qstats;           // optional GroupNorm quad sums [img][N_total/4][2] accumulated by the epilogue (mode 1)
@@ -131,26 +130,8 @@ bool tc_attn_supported(int T, int C);
 int tc_attn_plan_create(const TcAttnDesc& d, TcAttnPlan** out);
 void tc_attn_plan_destroy(TcAttnPlan* p);
 int tc_attn_launch(const TcAttnPlan* p, cudaStream_t st);
-// 3x3 convolution with GroupNorm (+SiLU) applied on load (gemm_tcg.cuh): fp16 operands, CTA pairs, W in {16, 32}
-struct TcgPlan;
-struct TcgDesc {
-  // 3x3 phase: up to two channel-concatenated NHWC sources (fp32 or fp16 elements), normalised on load
-  const void* a1; int C1; int a1_f16; const void* a2; int C2; int a2_f16;
-  const float* gn_scale; const float* gn_shift;   // [nimg][C1+C2] from launch_gn_coeff (both null: identity)
-  int act;                                        // SiLU after the affine
-  int H, W, nimg;
-  const float* w; int N_total;                    // fp16 [9][N_total][C1+C2]
-  // optional extra 1x1 phase (skip projection): out += [a3 | a4] w2^T, sources converted to fp16 on load
-  const void* a3; int C3; int a3_f16; const void* a4; int C4; int a4_f16; const float* w2;   // w2: fp16 [N_total][C3+C4]
-  double* qstats;
-  Epilogue epi;
-};
-bool tcg_supported(const TcgDesc& d, const char** why);
-int tcg_plan_create(const TcgDesc& d, TcgPlan** out);
-void tcg_plan_destroy(TcgPlan* p);
-int tcg_launch(const TcgPlan* p, cudaStream_t st);
 void tc_gemm_set_head(TcGemmPlan* p, float* out_nchw, const float* per_img_div, long long div_stride);   // per-call pointers of the NCHW head
-const char* tc_gemm_form(const TcGemmPlan* p);   // "pair256[-halo]" | "single256" | "single128" | "swap[-halo]"
+const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]"
 
 // ---- pc_update.cu -----------------------------------------------------------
 struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` elements

@@ -169,7 +169,7 @@ __global__ void step_increment_kernel(int* step) { pdl_wait(); pdl_trigger(); *s
 int apply_grid(const PhiloxMap& m) {
   const long long T = (long long)m.grid * m.block;
   const long long L = (m.numel + 4 * T - 1) / (4 * T);
-  return (int)std::min<long long>((T * L + 255) / 256, 148LL * 16);
+  return (int)std::min<long long>((T * L + 255) / 256, 132LL * 16);
 }
 
 }  // namespace

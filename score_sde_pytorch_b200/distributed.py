@@ -3,7 +3,7 @@
 The reference's only multi-GPU mechanism is ``torch.nn.DataParallel`` around the network
 (``models/utils.py:93``): every forward re-broadcasts all parameters (251 MB for the CIFAR-10
 NCSN++) to every GPU and gathers outputs on ``cuda:0`` while the loop, the RNG and the
-Langevin norms stay on one device.  Sample chains are independent, so the B200 layout is one
+Langevin norms stay on one device.  Sample chains are independent, so the layout is one
 process per GPU (``torchrun``), a full weight replica per rank broadcast **once** over
 NCCL/NVLink, per-rank batches with per-rank seeds, **no collective inside the loop**, and one
 final gather of the samples.
@@ -11,7 +11,7 @@ final gather of the samples.
 Batch coupling caveat: ``LangevinCorrector`` sets its step size from batch means of norms
 (``sampling.py:276-278``).  Each rank's sub-batch is therefore *defined* as its own reference
 batch: rank ``r`` equals the reference run with shape ``(B_r, ...)`` and seed ``seed + r``
-(SURVEY.md §8e).  ``shard_batch`` gives the per-rank sizes; ``rank_seed`` the seed rule.
+``shard_batch`` gives the per-rank sizes; ``rank_seed`` the seed rule.
 """
 import os
 

@@ -9,7 +9,7 @@ residual is reduced per image by ``b200_dsm_loss_f32`` (csrc/losses.cu); the per
 sigma, g^2) come from the SDE's own torch ops on ``[B]`` tensors, and ``t`` / ``z`` are drawn from torch's generator in the
 reference's order (``t`` first, then ``z``), so a CUDA seed gives the draws the reference would make on that device.
 The TRAINING step needs the network's backward pass and dropout, which the engine does not have: ``train=True`` raises
-``NotImplementedError`` (SURVEY section 8 f4; DESIGN.md section 8).  The optimizer plumbing is host logic and is mirrored so
+``NotImplementedError``.  The optimizer plumbing is host logic and is mirrored so
 that configs and checkpoints carry over.
 
 ``loss_fn(model, batch, t=None, z=None)``: the two extra arguments replace the internal draws (tests pin the loss to
@@ -48,7 +48,7 @@ def optimization_manager(config):
 
 
 def _no_training(what):
-  raise NotImplementedError(f'{what}: train=True needs the backward pass and dropout of the score network, which the sm_100a '
+  raise NotImplementedError(f'{what}: train=True needs the backward pass and dropout of the score network, which the sm_90a '
                             'engine does not implement (evaluation losses and sampling only)')
 
 

@@ -1,4 +1,4 @@
-"""NCSN++ score network backed by the sm_100a engine.
+"""NCSN++ score network backed by the sm_90a engine.
 
 Host-side mirror of ``models/ncsnpp.py:35-381``: ``NCSNpp(config)`` is an
 ``nn.Module`` registered as ``'ncsnpp'``; its parameters live in
@@ -8,7 +8,7 @@ Host-side mirror of ``models/ncsnpp.py:35-381``: ``NCSNpp(config)`` is an
 ``forward(x[B,C,H,W], time_cond[B]) -> [B,C,H,W]`` has the reference's meaning.
 
 The forward itself is not PyTorch: parameters are repacked once into the
-engine's blob (K-major, TF32-rounded where a layer runs on tcgen05) and every
+engine's blob (K-major, TF32-rounded where a layer runs on the tensor cores) and every
 call replays the engine's kernel sequence on the current CUDA stream through the
 C ABI (``include/scoresde_b200.h``).  CPU tensors are rejected — there is no CPU
 path in the product (the plain-PyTorch restatement lives in ``oracle/`` and is
@@ -24,7 +24,7 @@ from . import utils
 from .. import _lib
 
 PDL_DEFAULT = False
-HALO_DEFAULT = 'pairs'   # halo form of the 3x3 mainloop in the swapped AND the CTA-pair kernel (DESIGN.md section 4.13)
+HALO_DEFAULT = True      # halo form of the 3x3 mainloop in the swapped-operand kernel (csrc/gemm_tc.cu)
 
 _SUPPORTED = ("engine supports embedding_type in {'fourier','positional'}, conditional=True, resblock_type='biggan', "
               "fir in {True, False} (progressive_input='residual' needs fir=True), progressive in {'none','output_skip'}, "
@@ -114,8 +114,8 @@ def _pyramid_down(cin, cout):
 
 @utils.register_model(name='ncsnpp')
 class NCSNpp(nn.Module):
-  """NCSN++ model (engine-backed).  ``precision``: ``'tf32'`` (tcgen05 tensor cores on TF32-rounded
-  fp32 operands, default), ``'f16'`` (tcgen05 on fp16 operands: the same 11-bit significand as TF32
+  """NCSN++ model (engine-backed).  ``precision``: ``'tf32'`` (wgmma tensor cores on TF32-rounded
+  fp32 operands, default), ``'f16'`` (wgmma on fp16 operands: the same 11-bit significand as TF32
   with fp32 accumulation and fp32 activations between layers, half the operand traffic and twice the
   MMA rate) or ``'fp32'`` (strict fp32 on CUDA cores; validation mode)."""
 
@@ -142,21 +142,21 @@ class NCSNpp(nn.Module):
     self.lanes = int(getattr(m, 'lanes', lanes))   # 2: evaluate batches >= 128 as two half-batch lanes on two streams
     # per-engine execution options (fields of b200_ncsnpp_config; nothing is read from the environment)
     self.cuda_core_head = bool(getattr(m, 'cuda_core_head', False) if cuda_core_head is None else cuda_core_head)
-    # GroupNorm+SiLU as stand-alone streaming passes (True, default) or applied on load by the consuming convolution where
-    # supported (False; csrc/gemm_tcg.cuh).  Measured in the same run on the same B200: 62.41 vs 63.39 ms per PC step at
-    # batch 1024 (profiles/r02_g6_bench.json) - at the board's power cap the transform's arithmetic costs more than
-    # the 4.5 GB/evaluation of HBM traffic it removes, so the separate pass stays the default (DESIGN.md section 4.9).
+    # GroupNorm+SiLU of the tensor-core layers runs as a stand-alone streaming pass (True, default).  The convolution that
+    # applied it on load (False) is not part of this build, so False is rejected rather than silently ignored.
     # (2: separate passes also in front of the memory-bound few-channel convolutions of the nf = 16 networks, which
-    # otherwise always normalise on load in tf32 mode - csrc/conv_lowc.cu; kept for A/B tests)
+    # otherwise normalise on load in tf32 mode - csrc/conv_lowc.cu; kept for A/B tests)
     sg = getattr(m, 'separate_groupnorm', True) if separate_groupnorm is None else separate_groupnorm
-    self.separate_groupnorm = 2 if (not isinstance(sg, bool) and sg == 2) else bool(sg)
+    if not sg:
+      raise ValueError('NCSNpp: separate_groupnorm=False (GroupNorm applied on load by the tensor-core convolution) is not '
+                       'available in this build; use True (separate pass) or 2')
+    self.separate_groupnorm = 2 if (not isinstance(sg, bool) and sg == 2) else True
     # programmatic dependent launch between the kernels of a forward / PC iteration (common.cuh)
     self.pdl = bool(getattr(m, 'pdl', PDL_DEFAULT) if pdl is None else pdl)
-    # halo form of the 3x3 tensor-core mainloop (csrc/gemm_tc.cu, DESIGN.md section 4.13): 'pairs' (default) = in the swapped and
-    # the CTA-pair kernel, True = swapped kernel only, False = nine shifted tile loads per channel chunk (the round-1
-    # mainloop, kept for A/B); an int is the raw b200_ncsnpp_config.no_halo (tests: 2 | 8)
+    # halo form of the 3x3 tensor-core mainloop (csrc/gemm_tc.cu): True (default) = in the swapped-operand kernel, False =
+    # nine shifted tile loads per channel chunk (kept for A/B); an int is the raw b200_ncsnpp_config.no_halo (tests: 8)
     hv = getattr(m, 'halo', HALO_DEFAULT) if halo is None else halo
-    self.halo = hv if (hv == 'pairs' or (isinstance(hv, int) and not isinstance(hv, bool))) else bool(hv)   # int: raw b200_ncsnpp_config.no_halo
+    self.halo = hv if (isinstance(hv, int) and not isinstance(hv, bool)) else bool(hv)   # int: raw b200_ncsnpp_config.no_halo
     nf, ch_mult, nrb = m.nf, tuple(m.ch_mult), m.num_res_blocks
     L = len(ch_mult)
     all_res = [config.data.image_size // (2 ** i) for i in range(L)]
@@ -238,7 +238,7 @@ class NCSNpp(nn.Module):
     c.progressive_input = {'none': 0, 'residual': 1, 'input_skip': 2}[m.progressive_input.lower()]
     c.progressive = 1 if m.progressive.lower() == 'output_skip' else 0
     c.pdl = int(self.pdl)
-    c.no_halo = 2 if self.halo == 'pairs' else self.halo if (isinstance(self.halo, int) and not isinstance(self.halo, bool)) else int(not self.halo)
+    c.no_halo = self.halo if (isinstance(self.halo, int) and not isinstance(self.halo, bool)) else int(not self.halo)
     c.fir_taps = len(m.fir_kernel)
     for i, v in enumerate(m.fir_kernel):
       c.fir_kernel[i] = float(v)
@@ -363,7 +363,7 @@ class NCSNpp(nn.Module):
   def forward(self, x, time_cond, labels_uniform=False):
     if not x.is_cuda:
       raise RuntimeError('NCSNpp (score_sde_pytorch_b200) runs on CUDA devices only: there is no CPU path; '
-                         'move the model and inputs to a B200 (the PyTorch restatement in oracle/ is test-only)')
+                         'move the model and inputs to a CUDA device (the PyTorch restatement in oracle/ is test-only)')
     if x.dim() != 4 or x.shape[1] != self.config.data.num_channels or x.shape[2] != self.config.data.image_size \
         or x.shape[3] != self.config.data.image_size:
       raise RuntimeError(f'NCSNpp: input shape {tuple(x.shape)} does not match the configured image geometry')

@@ -5,7 +5,7 @@ Mirror of the reference's ``models/utils.py`` surface: ``register_model`` /
 (``:63-85``), ``create_model`` (``:88-94``), ``get_model_fn`` (``:97-126``),
 ``get_score_fn`` (``:129-178``) and the numpy flatten helpers (``:181-188``).
 
-Differences that are deliberate (B200-first, see DESIGN.md):
+Differences that are deliberate:
 
 * ``create_model`` does **not** wrap the model in ``torch.nn.DataParallel``
   (``models/utils.py:93``).  Multi-GPU sampling runs one process per GPU with

@@ -1,7 +1,7 @@
 """Host driver of the native predictor–corrector loop.
 
 ``match_pc_plan`` decides whether a ``(sde, model, predictor, corrector)``
-combination handed to :func:`sampling.get_pc_sampler` is one the sm_100a engine
+combination handed to :func:`sampling.get_pc_sampler` is one the sm_90a engine
 implements end to end; if so it returns a :class:`PcPlan` whose ``run(x)``
 executes all ``sde.N`` iterations on the device (one CUDA-graph replay per
 iteration, noise from the in-kernel Philox stream that reproduces

@@ -1,4 +1,4 @@
-"""``fused_leaky_relu`` / ``FusedLeakyReLU`` on the sm_100a library.
+"""``fused_leaky_relu`` / ``FusedLeakyReLU`` on the sm_90a library.
 
 Mirror of ``op/fused_act.py:20-97``: ``y = leaky_relu(x + bias[c], negative_slope) * scale`` with the bias broadcast over
 dim 1, differentiable to second order like the reference's ``FusedLeakyReLUFunction`` / ``...Backward`` pair: the first

@@ -1,4 +1,4 @@
-"""``upfirdn2d(input, kernel, up=1, down=1, pad=(0, 0))`` — FIR resampling on the sm_100a library.
+"""``upfirdn2d(input, kernel, up=1, down=1, pad=(0, 0))`` — FIR resampling on the sm_90a library.
 
 Same call surface and result as the reference op (``op/upfirdn2d.py:145-156``): ``input`` is NCHW,
 ``kernel`` a 2-D FIR, ``up``/``down`` integer factors, ``pad=(pad0, pad1)`` applied to both axes.

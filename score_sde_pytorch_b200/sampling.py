@@ -6,7 +6,7 @@ Mirror of the reference's ``sampling.py`` surface — registries (``:30-77``),
 ``shared_{predictor,corrector}_update_fn`` (``:333-352``), ``get_pc_sampler``
 (``:355-411``) and ``get_ode_sampler`` (``:414-485``) — with one structural
 change: ``pc_sampler(model)`` first asks :mod:`score_sde_pytorch_b200.native`
-whether ``(sde, predictor, corrector, model)`` is a combination the sm_100a
+whether ``(sde, predictor, corrector, model)`` is a combination the sm_90a
 engine implements (an engine-backed NCSN++ on a CUDA device with the
 reverse-diffusion / Euler–Maruyama / none predictor and the Langevin / none
 corrector).  If so the whole loop — both network evaluations, the in-kernel

@@ -1,4 +1,4 @@
-"""CPU tests for SURVEY 8 (f4): the losses oracle and the op-gradient oracle against goldens written by the REAL reference
+"""CPU tests for the losses oracle and the op-gradient oracle against goldens written by the REAL reference
 (tools/make_golden_f4.py), and the host logic of score_sde_pytorch_b200.losses (no device work)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""`-m gpu`: the DDPM++ family (SURVEY 8 f2, first variant; configs/vp/cifar10_ddpmpp_continuous.py): fir=False naive
+"""`-m gpu`: the DDPM++ family (configs/vp/cifar10_ddpmpp_continuous.py): fir=False naive
 2x resampling (up_or_down_sampling.py:59-69), sinusoidal positional embedding (layers.py:515-529, ncsnpp.py:242-247),
 no input pyramid, centred data, no division by sigma - through the same engine, against the oracle and against goldens
 written by the REAL reference (tools/make_golden_ddpmpp.py)."""

@@ -1,5 +1,5 @@
 """`-m gpu`: the NCSN++ engine (strict-fp32 execution mode) and the native PC loop against the oracle
-on the same device, same weights, same seeds.  TF32 / tcgen05 execution is covered in test_gpu_tc.py."""
+on the same device, same weights, same seeds.  TF32 / fp16 tensor-core execution is covered in test_gpu_tc.py."""
 import numpy as np
 import pytest
 import torch

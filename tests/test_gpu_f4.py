@@ -1,5 +1,5 @@
-"""`-m gpu`: SURVEY 8 (f4) - gradients of the two native ops (op/upfirdn2d.py:19-141, op/fused_act.py:20-72) through the
-package's autograd Functions on the sm_100a kernels, and the evaluation losses (losses.py:55-210, train=False) through
+"""`-m gpu`: gradients of the two native ops (op/upfirdn2d.py:19-141, op/fused_act.py:20-72) through the
+package's autograd Functions on the sm_90a kernels, and the evaluation losses (losses.py:55-210, train=False) through
 the engine, all against goldens written by the REAL reference (tools/make_golden_f4.py) and against the oracle."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""`-m gpu`: probability-flow ODE sampler with the state on the device (SURVEY 8 f3; sampling.py:414-485).
+"""`-m gpu`: probability-flow ODE sampler with the state on the device (sampling.py:414-485).
 
 The device solver (score_sde_pytorch_b200/ode.py + csrc/ode.cu) is held to
   * this package's own host loop over scipy.integrate.solve_ivp on the SAME engine network (`device_solver=False`): same

@@ -1,4 +1,4 @@
-"""`-m gpu`: the high-resolution NCSN++ family (SURVEY 8 f2, second variant): progressive='output_skip',
+"""`-m gpu`: the high-resolution NCSN++ family: progressive='output_skip',
 progressive_input='input_skip', Combine 'sum' (models/ncsnpp.py:163-166, 190-203, 289-292, 325-341, 366-367;
 layerspp.py:44-59) through the engine - against the oracle, against a golden written by the REAL reference
 (tools/make_golden_progressive.py), and at full size for the two reference configurations of the family."""
@@ -92,7 +92,7 @@ def test_few_channel_levels_groupnorm_on_load_matches_separate_passes(dev):
 def test_high_resolution_reference_configs_full_size(dev, name, precision):
   """configs/ve/celebahq_256_ncsnpp_continuous.py (65.6 M parameters, 256x256, seven levels) and
   configs/ve/ffhq_ncsnpp_continuous.py (105.8 M parameters, 1024x1024, eight levels, nf=16: the 16/32/64-channel levels run on
-  the few-channel TF32 MMA kernel, the rest on tcgen05), one evaluation at batch 1 against the strict-fp32 oracle."""
+  the few-channel TF32 MMA kernel, the rest on the wgmma kernels), one evaluation at batch 1 against the strict-fp32 oracle."""
   cfg = golden_config(name)
   model = seeded_model(cfg, precision=precision).to(dev)
   sd = {k: v.to(dev) for k, v in model.state_dict().items()}
@@ -111,7 +111,7 @@ def test_high_resolution_reference_configs_full_size(dev, name, precision):
 
 @pytest.mark.parametrize('precision', ['tf32', 'f16'])
 def test_deep_cifar10_variant_matches_oracle(dev, precision):
-  """configs/ve/cifar10_ncsnpp_deep_continuous.py: eight residual blocks per level (SURVEY 8 f2, "deep")."""
+  """configs/ve/cifar10_ncsnpp_deep_continuous.py: eight residual blocks per level ("deep")."""
   cfg = golden_config('cifar10_deep')
   model = seeded_model(cfg, precision=precision).to(dev)
   sd = {k: v.to(dev) for k, v in model.state_dict().items()}
@@ -126,7 +126,7 @@ def test_deep_cifar10_variant_matches_oracle(dev, precision):
 
 
 def test_baseline_config3_ddpmpp_celebahq256_subvp_ode_sampler(dev):
-  """BASELINE.json configs[3] at batch 1: DDPM++ cont. (fir=False, positional embedding) at 256x256 under the sub-VP SDE,
+  """Benchmark configuration 3 at batch 1: DDPM++ cont. (fir=False, positional embedding) at 256x256 under the sub-VP SDE,
   probability-flow ODE sampler with the state on the device.  One evaluation against the strict-fp32 oracle, then the
   device RK45 solve against this package's scipy host loop on the same network (looser tolerances than the default
   1e-5 keep the oracle-free comparison to a few dozen evaluations)."""
@@ -151,7 +151,7 @@ def test_baseline_config3_ddpmpp_celebahq256_subvp_ode_sampler(dev):
 
 
 def test_baseline_config4_ffhq1024_pc_sampler_steps(dev):
-  """BASELINE.json configs[4] at batch 1: NCSN++ FFHQ 1024x1024 VE-SDE PC sampler (reverse diffusion + Langevin) through
+  """Benchmark configuration 4 at batch 1: NCSN++ FFHQ 1024x1024 VE-SDE PC sampler (reverse diffusion + Langevin) through
   the native loop in tf32 mode, two iterations (four 1024x1024 evaluations) against the oracle loop on the same noise."""
   from score_sde_pytorch_b200 import native, sampling, sde_lib
   cfg = golden_config('ffhq_1024')

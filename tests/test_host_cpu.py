@@ -45,7 +45,7 @@ def test_generic_pc_loop_matches_reference_ve():
 
 
 def test_get_sampling_fn_vp_em_plumbing():
-  """BASELINE.json configs[0]-style plumbing: VP SDE, Euler-Maruyama predictor only, 20 steps, B=2, CPU."""
+  """Plumbing: VP SDE, Euler-Maruyama predictor only, 20 steps, B=2, CPU."""
   g = golden('pc_vp_tiny.npz')
   cfg = golden_config('tiny_vp')
   cfg.device = torch.device('cpu')
@@ -256,7 +256,7 @@ def test_ddpmpp_engine_param_table_has_the_reference_names_plus_the_frequency_ta
 
 
 def test_progressive_family_param_tables_match_module():
-  """output_skip / input_skip (SURVEY 8 f2): engine parameter table == module parameters for a small member and for the
+  """output_skip / input_skip: engine parameter table == module parameters for a small member and for the
   full-size CelebA-HQ-256 / FFHQ-1024 configurations (whose state_dict layouts tools/make_golden_progressive.py loads
   into the reference's constructor with strict=True: 65 574 549 and 105 785 896 parameters)."""
   for name, nparams in (('tiny_progressive', None), ('celebahq_256', 65574549), ('ffhq_1024', 105785896)):
@@ -298,17 +298,17 @@ def test_bench_reference_arm_prints_the_contract_line():
   import sys
   root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
   env = dict(os.environ, OMP_NUM_THREADS='1')      # what torchrun exports to every rank
-  out = subprocess.run([sys.executable, os.path.join(root, 'bench.py'), '--impl', 'reference', '--steps', '1', '--warmup', '0',
+  out = subprocess.run([sys.executable, os.path.join(root, 'bench.py'), '--impl', 'reference', '--steps', '5', '--warmup', '0',
                         '--cpu-batch', '1'], capture_output=True, text=True, timeout=900, env=env, cwd=root)
   assert out.returncode == 0, out.stderr[-2000:]
   line = json.loads(out.stdout.strip().splitlines()[-1])
   assert line['impl'] == 'reference' and line['unit'] == 'images/s' and line['higher_is_better'] is True
   assert line['metric'].startswith('PC-sampler images/sec') and line['value'] > 0 and line['n_gpus'] == 1
   cb = line['cpu_baseline']
-  # the UNMODIFIED reference from baseline/_ref (tools/install_ref.sh) when it is installed, else the oracle port
-  want = 'reference' if os.path.isdir(os.path.join(root, 'baseline', '_ref', 'models')) else 'port'
+  # the UNMODIFIED reference from oracle/_ref (oracle/install_ref.sh) when it is installed, else the oracle port
+  want = 'reference' if os.path.isdir(os.path.join(root, 'oracle', '_ref', 'models')) else 'port'
   assert cb['kind'] == want and cb['value'] == line['value'] and cb['cores'] >= 1 and 'PC iterations' in cb['sample']
-  assert line['steps'] >= 5 and len(cb['iter_seconds']) == line['steps']      # the median of >= 5 iterations is reported
+  assert line['steps'] == 5 and len(cb['iter_seconds']) == line['steps']      # --steps sets the timed iterations; their median is reported
   assert line['e2e'] == {'value': line['value'], 'unit': 'images/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0}
   if (os.cpu_count() or 1) >= 4:
     assert cb['cores'] > 1        # OMP_NUM_THREADS=1 from the launcher must not reduce the arm to one core
@@ -382,35 +382,17 @@ def test_parameter_list_matches_the_reference_order(name):
   assert mine == ref
 
 
-def test_profile_tooling_reads_the_committed_artifacts():
-  """The roofline block of bench.py takes `traffic` from profiles/traffic_f16.json (written by
-  tools/summarize_traffic.py from an ncu metrics pass); the launch-list summariser must keep parsing the committed CSV."""
-  import glob
-  import os
-  import subprocess
-  import sys
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  sys.path.insert(0, root)
-  import bench
-  t = bench.load_traffic('f16')
-  assert isinstance(t, int) and t > 10_000_000            # DRAM bytes per contraction launch
-  assert bench.load_traffic('no-such-precision') is None
-  csvs = sorted(glob.glob(os.path.join(root, 'profiles', '*launches_pc_step*_f16.csv')))
-  assert csvs, 'no committed launch list'
-  out = subprocess.run([sys.executable, os.path.join(root, 'tools', 'summarize_launches.py'), csvs[-1]],
-                       capture_output=True, text=True, timeout=120)
-  assert out.returncode == 0 and 'gemm_tc' in out.stdout and 'gn_apply' in out.stdout
-
-
 def test_execution_options_reach_the_native_config():
   """Per-engine options are fields of b200_ncsnpp_config (nothing is read from the environment).  `halo`: the package
-  default is the halo form in the swapped AND the CTA-pair kernel (no_halo = 2); True / False / raw ints map as documented
+  default is no_halo = 0 (halo form in the swapped kernel); True / False / raw ints map as documented
   in include/scoresde_b200.h."""
   from score_sde_pytorch_b200.models.ncsnpp import NCSNpp
   cfg = golden_config('tiny')
-  want = {None: 2, 'pairs': 2, True: 0, False: 1, 2 | 8: 10, 6: 6}
+  want = {None: 0, True: 0, False: 1, 8: 8, 2 | 8: 10, 6: 6}
   for halo, no_halo in want.items():
     m = NCSNpp(cfg) if halo is None else NCSNpp(cfg, halo=halo)
     assert m._native_config().no_halo == no_halo, (halo, m._native_config().no_halo)
-  c = NCSNpp(cfg, precision='f16', separate_groupnorm=False, pdl=True, cuda_core_head=True)._native_config()
-  assert (c.precision, c.separate_groupnorm, c.pdl, c.cuda_core_head) == (2, 0, 1, 1)
+  c = NCSNpp(cfg, precision='f16', separate_groupnorm=2, pdl=True, cuda_core_head=True)._native_config()
+  assert (c.precision, c.separate_groupnorm, c.pdl, c.cuda_core_head) == (2, 2, 1, 1)
+  with pytest.raises(ValueError):           # GroupNorm on load by the tensor-core convolution is not in this build
+    NCSNpp(cfg, precision='f16', separate_groupnorm=False)

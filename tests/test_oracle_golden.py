@@ -133,7 +133,7 @@ def test_pc_sampler_oracle_matches_reference_ancestral_and_ald():
 
 
 def test_pc_sampler_oracle_matches_reference_ddpmpp():
-  """DDPM++ (SURVEY 8 f2; tools/make_golden_ddpmpp.py): the config's own sampler - Euler-Maruyama, no corrector -
+  """DDPM++ (tools/make_golden_ddpmpp.py): the config's own sampler - Euler-Maruyama, no corrector -
   under the VP and sub-VP SDEs, through the reference's get_pc_sampler on the reference's NCSNpp(fir=False,
   embedding_type='positional')."""
   g = golden('pc_ddpmpp_tiny.npz')
@@ -151,7 +151,7 @@ def test_pc_sampler_oracle_matches_reference_ddpmpp():
 
 @pytest.mark.parametrize('case', ['ve', 'vp', 'subvp'])
 def test_ode_sampler_oracle_matches_reference(case):
-  """SURVEY 8 f3 pin (tools/make_golden_ode.py): the reference's get_ode_sampler (scipy RK45, rtol = atol = 1e-5) on the
+  """ODE sampler pin (tools/make_golden_ode.py): the reference's get_ode_sampler (scipy RK45, rtol = atol = 1e-5) on the
   reference's own networks; the sub-VP case with the one-step denoise."""
   g = golden('ode_tiny.npz')
   name, sde, eps, denoise = {'ve': ('tiny', SO.VE(0.01, 50, 1000), 1e-5, False),

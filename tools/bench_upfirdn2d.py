@@ -1,8 +1,8 @@
 """INTEGRATION.md binding B1 measured: `b200_upfirdn2d_f32` in the reference's own tensor convention ([N*C, H, W, 1],
-op/upfirdn2d.py:99) against the reference's JIT-compiled `upfirdn2d_op` (op/upfirdn2d_kernel.cu, from baseline/_ref,
+op/upfirdn2d.py:99) against the reference's JIT-compiled `upfirdn2d_op` (op/upfirdn2d_kernel.cu, from oracle/_ref,
 unmodified) on the same GPU tensors, for the three parameterisations NCSN++ uses.  Prints one markdown table:
 
-    python tools/bench_upfirdn2d.py [--md profiles/rNN_upfirdn2d_b1.md]
+    python tools/bench_upfirdn2d.py [--md OUT.md]
 """
 import argparse
 import os

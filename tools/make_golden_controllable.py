@@ -1,4 +1,4 @@
-"""Golden fixtures for controllable generation (SURVEY 8 f4, second half; controllable_generation.py:8-198) from the REAL
+"""Golden fixtures for controllable generation (controllable_generation.py:8-198) from the REAL
 reference: get_pc_inpainter and get_pc_colorizer with the reverse-diffusion predictor + Langevin corrector under the VE
 SDE (N = 12) on the reference's own tiny NCSNpp, CPU, fixed seeds.  controllable_tiny.npz: data, mask, inpainted,
 gray, colorized.

@@ -1,4 +1,4 @@
-"""Golden fixtures for the DDPM++ family (SURVEY 8 f2, configs/vp/cifar10_ddpmpp_continuous.py) from the REAL reference,
+"""Golden fixtures for the DDPM++ family (configs/vp/cifar10_ddpmpp_continuous.py) from the REAL reference,
 same recipe as tools/make_golden.py: this repository's deterministic weights are loaded into the reference's NCSNpp with
 load_state_dict(strict=True) (fir=False naive resampling, positional embedding, no input pyramid), then
 

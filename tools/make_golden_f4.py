@@ -1,4 +1,4 @@
-"""Golden fixtures for SURVEY 8 (f4) from the REAL reference, run on CPU (same recipe as tools/make_golden.py):
+"""Golden fixtures for the losses and op gradients from the REAL reference, run on CPU (same recipe as tools/make_golden.py):
 
   f4_op_grads.npz   first and second derivatives of the reference's two native ops through its own CPU forms under autograd
                     (op/upfirdn2d.py:159-200 `upfirdn2d_native`; op/fused_act.py:85-93) - what its CUDA autograd Functions
@@ -119,7 +119,7 @@ def loss_goldens(sde_lib, mutils):
 
 class StandIn(torch.nn.Module):
   """A deterministic stand-in score model for the SMLD loss: the reference's own positional-embedding VE network raises a
-  dtype error on current PyTorch (SURVEY Appendix C-4), and the loss arithmetic does not care what the model is."""
+  dtype error on current PyTorch , and the loss arithmetic does not care what the model is."""
 
   def forward(self, x, labels):
     return 0.3 * torch.flip(x, dims=(3,)) + (0.001 * labels.float())[:, None, None, None] * x

@@ -1,4 +1,4 @@
-"""Golden fixtures for the probability-flow ODE sampler (SURVEY 8 f3, sampling.py:414-485) from the REAL reference:
+"""Golden fixtures for the probability-flow ODE sampler (sampling.py:414-485) from the REAL reference:
 get_ode_sampler (scipy RK45, rtol = atol = 1e-5) on the reference's own NCSNpp with this repository's deterministic
 weights, on CPU, for a fixed latent z.  ode_tiny.npz: per case z, samples, nfe.
 

@@ -1,4 +1,4 @@
-"""Golden fixtures for the high-resolution NCSN++ family (SURVEY 8 f2: progressive='output_skip',
+"""Golden fixtures for the high-resolution NCSN++ family (progressive='output_skip',
 progressive_input='input_skip', Combine 'sum'; configs/ve/{ffhq,celebahq_256}_ncsnpp_continuous.py) from the REAL
 reference, same recipe as tools/make_golden.py.  One small member of the family (three levels, 32x32, FIR resampling): forward at batch 2 with every all_modules[i] activation; plus the state_dict key check of the full-size
 CelebA-HQ-256 and FFHQ-1024 configurations (load_state_dict(strict=True) into the reference's constructor, no forward).

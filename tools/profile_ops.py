@@ -1,5 +1,5 @@
 """Per-op device time of one network evaluation (CUDA events around every launch, run serially on one
-stream), grouped by shape label:  python tools/profile_ops.py --batch 1024 [--md profiles/rNN_ops.md]"""
+stream), grouped by shape label:  python tools/profile_ops.py --batch 1024 [--md OUT.md]"""
 import argparse
 import collections
 import ctypes
