@@ -102,7 +102,8 @@ B200_API int b200_gemm_nt_f32(const float* a, long long lda, int a_batch_rows, c
  * models/up_or_down_sampling.py, op/) for configurations with Fourier embedding,
  * (or positional) embedding, BigGAN residual blocks, FIR or naive resampling, progressive in {'none','output_skip'}
  * and progressive_input in {'none','residual','input_skip'} (Combine method 'sum').  forward(x[B,C,H,W], time_cond[B]) -> [B,C,H,W]
- * like NCSNpp.forward (models/ncsnpp.py:232). */
+ * like NCSNpp.forward (models/ncsnpp.py:232).  With family = 1 the same handle type runs the DDPM network
+ * (models/ddpm.py:39-181, DDPM.forward :110-181); every entry point below, the PC loop included, works unchanged. */
 typedef struct b200_ncsnpp b200_ncsnpp_t;
 
 typedef struct {
@@ -142,6 +143,14 @@ typedef struct {
                                  * row-major launches of shapes with a halo form walk K in that form's order, so plans of different batch
                                  * sizes agree bit for bit (tests).  Swapped-form results are bit-identical in every mode (same products,
                                  * same order). */
+  int family;                   /* 0 = NCSN++ / DDPM++ (models/ncsnpp.py, the default); 1 = DDPM (models/ddpm.py:39-181): ResnetBlockDDPM
+                                 * with the NIN_0 skip (layers.py:619-662), AttnBlock (:558-581), Downsample / Upsample with_conv
+                                 * (:584-616), residual scale 1, GroupNorm with 32 groups everywhere (channel counts must be multiples
+                                 * of 32), sinusoidal time embedding through the "pos_freqs" pseudo-parameter.  Family 1 reads
+                                 * image_size, num_channels, nf, num_res_blocks, num_levels, ch_mult, num_attn_resolutions,
+                                 * attn_resolutions, centered and the execution fields (precision ... no_halo); it requires
+                                 * conditional = 1 and scale_by_sigma = 0, and ignores skip_rescale, progressive_input, progressive,
+                                 * fir_taps / fir_kernel, naive_resample and embedding_type. */
 } b200_ncsnpp_config;
 
 B200_API int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out);

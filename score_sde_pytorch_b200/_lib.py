@@ -32,7 +32,7 @@ class NcsnppConfig(ctypes.Structure):
               ('precision', c_int), ('keep_activations', c_int), ('lanes', c_int),
               ('cuda_core_head', c_int), ('separate_groupnorm', c_int),
               ('embedding_type', c_int), ('naive_resample', c_int), ('progressive', c_int), ('pdl', c_int),
-              ('no_halo', c_int)]
+              ('no_halo', c_int), ('family', c_int)]
 
 
 class PcConfig(ctypes.Structure):

@@ -195,6 +195,77 @@ def tiny_progressive(nf=32, image_size=32, num_res_blocks=1, ch_mult=(1, 1, 2), 
   return c
 
 
+def vp_cifar10_ddpm_continuous():
+  """``configs/vp/ddpm/cifar10_continuous.py`` — DDPM cont. (VP): the ``models/ddpm.py`` network, centred data,
+  Euler-Maruyama predictor, no corrector."""
+  c = cifar10_defaults()
+  c.training.sde = 'vpsde'
+  c.training.continuous = True
+  c.training.reduce_mean = True
+  c.sampling.method = 'pc'
+  c.sampling.predictor = 'euler_maruyama'
+  c.sampling.corrector = 'none'
+  c.data.centered = True
+  m = c.model
+  m.name = 'ddpm'
+  m.scale_by_sigma = False
+  m.ema_rate = 0.9999
+  m.normalization = 'GroupNorm'
+  m.nonlinearity = 'swish'
+  m.nf = 128
+  m.ch_mult = (1, 2, 2, 2)
+  m.num_res_blocks = 2
+  m.attn_resolutions = (16,)
+  m.resamp_with_conv = True
+  m.conditional = True
+  return c
+
+
+def subvp_cifar10_ddpm_continuous():
+  """``configs/subvp/cifar10_ddpm_continuous.py`` — the same network under the sub-VP SDE."""
+  c = vp_cifar10_ddpm_continuous()
+  c.training.sde = 'subvpsde'
+  return c
+
+
+def vp_cifar10_ddpm():
+  """``configs/vp/ddpm/cifar10.py`` — discrete-time DDPM (``continuous=False``), ancestral sampling.  Samples through the
+  generic host loop over the engine network."""
+  c = vp_cifar10_ddpm_continuous()
+  c.training.continuous = False
+  c.sampling.predictor = 'ancestral_sampling'
+  return c
+
+
+def vp_celebahq_256_ddpm():
+  """``configs/vp/ddpm/celebahq.py`` over ``configs/default_lsun_configs.py``: 256x256, ch_mult (1,1,2,2,4,4), two blocks
+  per level, attention at 16x16, discrete time, ancestral sampling."""
+  c = vp_cifar10_ddpm()
+  c.data.dataset = 'CelebAHQ'
+  c.data.image_size = 256
+  c.training.batch_size = 64
+  c.eval.batch_size = 512
+  m = c.model
+  m.sigma_max = 378          # configs/default_lsun_configs.py:51-56
+  m.dropout = 0.
+  m.num_scales = 1000        # configs/vp/ddpm/celebahq.py
+  m.ch_mult = (1, 1, 2, 2, 4, 4)
+  m.num_res_blocks = 2
+  m.attn_resolutions = (16,)
+  return c
+
+
+def tiny_ddpm(nf=32, image_size=16, num_res_blocks=1, ch_mult=(1, 2), attn_resolutions=(8,)):
+  """A small DDPM of the same family (test fixture sized; not a reference config)."""
+  c = vp_cifar10_ddpm_continuous()
+  c.model.nf = nf
+  c.model.ch_mult = tuple(ch_mult)
+  c.model.num_res_blocks = num_res_blocks
+  c.model.attn_resolutions = tuple(attn_resolutions)
+  c.data.image_size = image_size
+  return c
+
+
 def subvp_celebahq_256_ddpmpp_continuous():
   """DDPM++ cont. CelebA-HQ 256 sub-VP.  The reference ships no such config file; it is composed from ``configs/subvp/cifar10_ddpmpp_continuous.py`` (DDPM++: ``fir=False``, positional
   embedding, no pyramids, sub-VP SDE, Euler-Maruyama predictor) with the 256-pixel data / ``ch_mult`` fields of

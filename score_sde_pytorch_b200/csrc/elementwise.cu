@@ -945,6 +945,23 @@ int launch_nhwc_to_nchw(const float* src, float* dst, int B, int HW, int C, cuda
   return 0;
 }
 
+// operand-format copy of an fp32 activation (the DDPM Downsample convolution reads a block output directly)
+__global__ void __launch_bounds__(256) store_operand_kernel(const float4* __restrict__ x, float* __restrict__ y, long long n4, int mode) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x)
+    store_operand4(y, 4 * i, __ldg(x + i), mode);
+}
+int launch_store_operand(const float* x, float* y, long long n, int mode, cudaStream_t st) {
+  B200_REQUIRE(n % 4 == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) % 16) == 0,
+               "store_operand: %lld elements / pointer alignment not float4-aligned", n);
+  const long long n4 = n / 4;
+  if (n4 == 0) return 0;
+  launch_kernel(store_operand_kernel, dim3((int)std::min<long long>((n4 + 255) / 256, 132LL * 16)), dim3(256), 0, st,
+                reinterpret_cast<const float4*>(x), y, n4, mode);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
 // dst[tap*dt + o*dO + i] = src[o*so + i*si + tap*st]  (OIHW conv weights: so=I*R*S, si=R*S, st=1;
 // NIN W[in][out]: taps=1, so=1, si=out).  Default destination [tap][o][i] (dt=O*I, dO=I); the
 // flat-K packing of the input convolution uses dt=I, dO=row pitch.  Optional TF32 rounding.

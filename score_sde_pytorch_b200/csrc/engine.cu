@@ -19,7 +19,8 @@ using namespace b200;
 
 namespace {
 
-enum ModKind { M_FOURIER, M_LINEAR, M_CONV_IN, M_RESBLOCK, M_ATTN, M_PYR_DOWN, M_GN_OUT, M_CONV_OUT, M_COMBINE };
+// M_DOWN / M_UP: the DDPM family's Downsample / Upsample with_conv (layers.py:584-616)
+enum ModKind { M_FOURIER, M_LINEAR, M_CONV_IN, M_RESBLOCK, M_ATTN, M_PYR_DOWN, M_GN_OUT, M_CONV_OUT, M_COMBINE, M_DOWN, M_UP };
 enum PackKind { PK_COPY = 0, PK_CONV = 1, PK_NIN = 2, PK_CONV_FLAT32 = 3, PK_CONV_PAD128 = 4 };
 
 struct Param {
@@ -161,8 +162,14 @@ bool tc_ok(const b200_ncsnpp* e, int C1, int C2, int Cout, int H, int W, int tap
 
 int build_graph(b200_ncsnpp* e) {
   const b200_ncsnpp_config& c = e->cfg;
+  const bool ddpm = c.family == 1;
   B200_REQUIRE(c.num_levels >= 1 && c.num_levels <= 8, "ncsnpp: num_levels=%d out of range", c.num_levels);
   B200_REQUIRE(c.nf % 4 == 0 && c.nf >= 8, "ncsnpp: nf=%d must be a multiple of 4", c.nf);
+  if (ddpm) {   // every GroupNorm has 32 groups (layers.py:562, 625, 633; ddpm.py:104)
+    B200_REQUIRE(c.nf % 32 == 0, "ddpm: nf=%d must be a multiple of 32 (GroupNorm with 32 groups)", c.nf);
+    for (int i = 0; i < c.num_levels; ++i)
+      B200_REQUIRE(c.ch_mult[i] >= 1 && (c.nf * c.ch_mult[i]) % 32 == 0, "ddpm: level %d has %d channels, not a multiple of 32", i, c.nf * c.ch_mult[i]);
+  }
   B200_REQUIRE(c.conditional, "ncsnpp: unconditional models are not supported by the engine");
   B200_REQUIRE(c.fir_taps >= 1 && c.fir_taps <= 8, "ncsnpp: fir kernel length %d unsupported", c.fir_taps);
   B200_REQUIRE((c.image_size >> (c.num_levels - 1)) >= 1 && c.image_size % (1 << (c.num_levels - 1)) == 0,
@@ -219,6 +226,8 @@ int build_graph(b200_ncsnpp* e) {
   { Mod m; m.kind = M_LINEAR; m.index = cur(); m.cin1 = 4 * nf; m.cout = 4 * nf;
     m.w = add_param(e, nm("weight"), {4 * nf, 4 * nf}, PK_COPY, 0, 0, 0, 0); m.b = add_param(e, nm("bias"), {4 * nf}, PK_COPY, 0, 0, 0, 0); e->mods.push_back(m); }
 
+  // NCSN++: ResnetBlockBigGANpp (layerspp.py:214-274); DDPM: ResnetBlockDDPM (layers.py:619-662), whose skip projection is
+  // NIN_0 (W [in][out], packed like a 1x1 convolution) instead of Conv_2, and which never resamples
   auto add_resblock = [&](int cin1, int cin2, int cout, int up, int down, int res_in) {
     Mod m; m.kind = M_RESBLOCK; m.index = cur();
     const int cin = cin1 + cin2;
@@ -241,10 +250,22 @@ int build_graph(b200_ncsnpp* e) {
     m.gn1b = add_param(e, nm("GroupNorm_1.bias"), {cout}, PK_COPY, 0, 0, 0, 0);
     m.c1w = add_param(e, nm("Conv_1.weight"), {cout, cout, 3, 3}, PK_CONV, 9, cout, cout, m.tc1 ? om : 0);
     m.c1b = add_param(e, nm("Conv_1.bias"), {cout}, PK_COPY, 0, 0, 0, 0);
-    if (m.has_conv2) {
+    if (m.has_conv2 && ddpm) {
+      m.c2w = add_param(e, nm("NIN_0.W"), {cin, cout}, PK_NIN, 1, cout, cin, m.tc2 ? om : 0);
+      m.c2b = add_param(e, nm("NIN_0.b"), {cout}, PK_COPY, 0, 0, 0, 0);
+    } else if (m.has_conv2) {
       m.c2w = add_param(e, nm("Conv_2.weight"), {cout, cin, 1, 1}, PK_CONV, 1, cout, cin, m.tc2 ? om : 0);
       m.c2b = add_param(e, nm("Conv_2.bias"), {cout}, PK_COPY, 0, 0, 0, 0);
     }
+    e->mods.push_back(m);
+  };
+  // DDPM Downsample (pad (0,1,0,1) + 3x3 stride-2 VALID conv) and Upsample (nearest 2x + 3x3 conv): Conv_0 is C -> C
+  auto add_resample = [&](ModKind kind, int C, int res_in) {
+    Mod m; m.kind = kind; m.index = cur(); m.cin1 = C; m.cout = C; m.res = res_in;
+    const int ro = kind == M_UP ? 2 * res_in : res_in / 2;
+    m.tc0 = tc_ok(e, C, 0, C, ro, ro, 9);
+    m.w = add_param(e, nm("Conv_0.weight"), {C, C, 3, 3}, PK_CONV, 9, C, C, m.tc0 ? om : 0);
+    m.b = add_param(e, nm("Conv_0.bias"), {C}, PK_COPY, 0, 0, 0, 0);
     e->mods.push_back(m);
   };
   auto add_attn = [&](int C, int res) {
@@ -294,7 +315,8 @@ int build_graph(b200_ncsnpp* e) {
       hs_c.push_back(in_ch);
     }
     if (lvl != L - 1) {
-      add_resblock(in_ch, 0, in_ch, 0, 1, all_res[lvl]);
+      if (ddpm) add_resample(M_DOWN, in_ch, all_res[lvl]);
+      else add_resblock(in_ch, 0, in_ch, 0, 1, all_res[lvl]);
       if (c.progressive_input == 2) {
         // Combine(dim1 = image channels, dim2 = in_ch, method 'sum') (layerspp.py:44-59, ncsnpp.py:163-166): Conv_0 is a 1x1
         Mod m; m.kind = M_COMBINE; m.index = cur(); m.cin1 = ch; m.cout = in_ch; m.res = all_res[lvl] / 2;
@@ -338,7 +360,10 @@ int build_graph(b200_ncsnpp* e) {
         m.w = add_param(e, nm("weight"), {ch, in_ch, 3, 3}, PK_CONV, 9, ch, in_ch, 0);
         m.b = add_param(e, nm("bias"), {ch}, PK_COPY, 0, 0, 0, 0); e->mods.push_back(m); }
     }
-    if (lvl != 0) add_resblock(in_ch, 0, in_ch, 1, 0, all_res[lvl]);
+    if (lvl != 0) {
+      if (ddpm) add_resample(M_UP, in_ch, all_res[lvl]);
+      else add_resblock(in_ch, 0, in_ch, 1, 0, all_res[lvl]);
+    }
   }
   B200_REQUIRE(hs_c.empty(), "ncsnpp: internal skip-stack mismatch");
   if (c.progressive != 1) {
@@ -426,8 +451,10 @@ struct Builder {
     name("gn_quad_stats %d @%d", t.C, t.H);
     op(1, [=](cudaStream_t st) { return launch_gn_quad_stats(tt.p, tt.C, Bc, tt.H * tt.W, tt.qs, st, /*qsums_zeroed=*/true); }, 2);
   }
+  // GroupNorm group count: min(C/4, 32) in NCSN++ (layerspp.py:219, 235), 32 everywhere in DDPM (layers.py:562, 625, 633)
+  int groups(int C) const { return e->cfg.family == 1 ? 32 : std::min(C / 4, 32); }
   void gn(Tensor& x1, Tensor& x2, int pgw, int pgb, int act, int round, Tensor y, float* raw) {
-    const int C = x1.C + x2.C, G = std::min(C / 4, 32), HW = x1.H * x1.W;
+    const int C = x1.C + x2.C, G = groups(C), HW = x1.H * x1.W;
     if ((C / G) % 4 != 0) {
       // groups that are not whole channel quads (C = 192 -> 6 channels per group): the generic two-kernel path
       if (x1.f16 || x2.f16) { set_error("ncsnpp: GroupNorm with %d-channel groups on an fp16 tensor", C / G); rc = 2; return; }
@@ -451,7 +478,7 @@ struct Builder {
   // ---- GroupNorm coefficient tables for the few-channel convolutions that normalise while staging their input ----
   struct Coef { float* scale = nullptr; float* shift = nullptr; long long bytes = 0; };
   Coef gncoef(Tensor& x1, Tensor& x2, int pgw, int pgb) {
-    const int C = x1.C + x2.C, G = std::min(C / 4, 32), HW = x1.H * x1.W;
+    const int C = x1.C + x2.C, G = groups(C), HW = x1.H * x1.W;
     ensure_qs(x1); ensure_qs(x2);
     Coef c;
     c.scale = falloc(2LL * B * C, &c.bytes); c.shift = c.scale + (long long)B * C;
@@ -623,10 +650,10 @@ struct Builder {
     const bool h1_f16 = om == 2 && m.tc0 && m.tc1 && fused_stats && (Ho * Ho) % 32 == 0 && (m.cout % 128 == 0);
     // few-channel levels (TF32 mode): both 3x3 convolutions normalise their input while they stage it, so neither
     // GroupNorm writes a tensor (quad-aligned groups only: the coefficient kernel works on channel quads)
-    const int G0 = std::min(Cin / 4, 32);
+    const int G0 = groups(Cin), G1 = groups(m.cout);
     const bool lc0 = lowc_gn && !m.tc0 && !resample && !x1.f16 && !x2.f16 && Cin % G0 == 0 && (Cin / G0) % 4 == 0 && x1.C % 4 == 0 &&
                      lowc_ok(x1.C, x2.C, m.cout, H, 9);
-    const bool lc1 = lowc_gn && !m.tc1 && lowc_ok(m.cout, 0, m.cout, Ho, 9);
+    const bool lc1 = lowc_gn && !m.tc1 && m.cout % G1 == 0 && (m.cout / G1) % 4 == 0 && lowc_ok(m.cout, 0, m.cout, Ho, 9);
     Tensor a0, raw;   // raw: operand-format copy of the (concatenated) block input for the tensor-core skip conv
     if (!lc0) {
       a0 = talloc(Cin, H, H);
@@ -774,6 +801,44 @@ struct Builder {
     return out;
   }
 
+  // DDPM Downsample(with_conv) (layers.py:599-616): F.pad(x, (0,1,0,1)) then a 3x3 stride-2 VALID convolution.  The
+  // convolution reads the unpadded input: the taps of the last output row / column that fall on row / column H are the
+  // padding zeros (TMA's out-of-bounds fill on the tensor cores, the bounds check of the CUDA-core kernel otherwise).
+  Tensor downsample(const Mod& m, Tensor& x) {
+    const int H = x.H, Ho = H / 2;
+    Tensor out = talloc(m.cout, Ho, Ho);
+    if (m.tc0) {
+      // the block output is fp32; the tensor cores read it in the operand format (TF32 grid / fp16)
+      Tensor xo = talloc(x.C, H, H);
+      const float* src = x.p; float* dst = xo.p; const long long n = (long long)B * H * H * x.C; const int omc = om;
+      name("operand copy %d @%d", x.C, H);
+      next_bytes = (double)n * (4.0 + (om == 2 ? 2.0 : 4.0));
+      op(1, [=](cudaStream_t st) { return launch_store_operand(src, dst, n, omc, st); }, 6);
+      conv(true, xo, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true, /*stride=*/2, /*Hin=*/H);
+      tfree(xo);
+    } else {
+      SimtConv s; memset(&s, 0, sizeof(s));
+      s.x1 = x.p; s.C1 = x.C; s.in_scale = 1.f; s.H = H; s.W = H; s.R = s.S = 3; s.stride = 2; s.pad = 0;
+      s.OH = Ho; s.OW = Ho; s.nbatch = B; s.a_batched = 1; s.w = e->W(m.w); s.N = m.cout;
+      s.epi.bias = e->W(m.b); s.epi.scale = 1.f; s.epi.rows_per_img = Ho * Ho; s.epi.out = out.p; s.epi.ld_out = m.cout;
+      name("conv3x3 s2 %d->%d @%d [cuda-core]", x.C, m.cout, Ho);
+      op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
+    }
+    return out;
+  }
+
+  // DDPM Upsample(with_conv) (layers.py:584-596): nearest 2x (the 2x2 box upfirdn2d, written in the convolution's operand
+  // format) then a 3x3 'same' convolution
+  Tensor upsample(const Mod& m, Tensor& x) {
+    const int H = x.H, Ho = 2 * H;
+    Tensor u = talloc(x.C, Ho, Ho);
+    fir(x.p, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, u.p, 1.f, /*box=*/true);
+    Tensor out = talloc(m.cout, Ho, Ho);
+    conv(m.tc0, u, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true);
+    tfree(u);
+    return out;
+  }
+
   int build() {
     const b200_ncsnpp_config& c = e->cfg;
     const int nf = c.nf, R = c.image_size, ch = c.num_channels, sumC = e->sumC;
@@ -853,7 +918,7 @@ struct Builder {
       }
       if (lvl != L - 1) {
         const Mod& m = e->mods[mi++];
-        Tensor none; Tensor h = resblock(m, hs.back(), none); if (rc) return rc;
+        Tensor none; Tensor h = m.kind == M_DOWN ? downsample(m, hs.back()) : resblock(m, hs.back(), none); if (rc) return rc;
         tap(m.index, h);
         if (c.progressive_input == 2) {
           // input_skip (ncsnpp.py:289-292): the image pyramid is downsampled (no parameters) and a 1x1 convolution of it is
@@ -967,7 +1032,9 @@ struct Builder {
         opyr = dst; opyr_bytes = nb;
       }
       if (lvl != 0) {
-        Tensor none; const Mod& m = e->mods[mi++]; Tensor h2 = resblock(m, h, none); if (rc) return rc; tfree(h); h = h2; tap(m.index, h);
+        Tensor none; const Mod& m = e->mods[mi++];
+        Tensor h2 = m.kind == M_UP ? upsample(m, h) : resblock(m, h, none); if (rc) return rc;
+        tfree(h); h = h2; tap(m.index, h);
       }
     }
     // ---- output head (ncsnpp.py:371-379); with output_skip the pyramid already is the output ----
@@ -1052,8 +1119,22 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
   B200_REQUIRE(cfg && out, "ncsnpp_create: null argument");
   B200_REQUIRE(cfg->separate_groupnorm != 0, "ncsnpp_create: separate_groupnorm = 0 (GroupNorm applied on load by the tensor-core "
                "convolution) is not available in this build; use 1 or 2");
+  B200_REQUIRE(cfg->family == 0 || cfg->family == 1, "ncsnpp_create: family=%d unknown (0 NCSN++, 1 DDPM)", cfg->family);
+  if (cfg->family == 1) {
+    B200_REQUIRE(cfg->conditional, "ncsnpp_create: DDPM (family 1) needs conditional = 1 (the reference's own constructor fails "
+                 "without time conditioning, models/ddpm.py:58-71)");
+    B200_REQUIRE(!cfg->scale_by_sigma, "ncsnpp_create: DDPM (family 1) with scale_by_sigma = 1 (configs/ve/cifar10_ddpm.py) is not "
+                 "supported by the engine");
+  }
   b200_ncsnpp* e = new b200_ncsnpp();
   e->cfg = *cfg;
+  if (cfg->family == 1) {
+    // the fields DDPM ignores take the values that describe it on the shared paths: residual scale 1, no pyramids,
+    // sinusoidal embedding (ddpm.py:116), and a unit FIR that no DDPM layer reads
+    b200_ncsnpp_config& c = e->cfg;
+    c.skip_rescale = 0; c.progressive_input = 0; c.progressive = 0; c.embedding_type = 1; c.naive_resample = 1;
+    c.fir_taps = 1; c.fir_kernel[0] = 1.f;
+  }
   if (int r = build_graph(e)) { delete e; return r; }
   *out = e;
   return 0;

@@ -33,6 +33,8 @@ int launch_linear_rows(const float* x, long long ldx, const float* W, const floa
                        int K, int act_in, float* y, long long ldy, cudaStream_t st);
 int launch_fill_from_table(const float* table, const int* step, float* dst, int n, cudaStream_t st);
 int launch_nhwc_to_nchw(const float* src, float* dst, int B, int HW, int C, cudaStream_t st);
+// y = x in tensor-core operand format `mode` (store_operand4: 1 TF32 grid, 2 fp16); n % 4 == 0, 16-byte aligned pointers
+int launch_store_operand(const float* x, float* y, long long n, int mode, cudaStream_t st);
 int launch_pack_weight(const float* src, float* dst, int taps, int O, int I, long long so, long long si,
                        long long stp, int round_out, cudaStream_t st, long long dt = 0, long long dO = 0);
 int launch_im2col3x3_nchw(const float* x, float* patches, int B, int C, int Hin, int Win, int H, int W, int stride,

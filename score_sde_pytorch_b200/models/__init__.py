@@ -1,3 +1,4 @@
-"""Score models.  Importing the package registers ``'ncsnpp'`` (``models/utils.register_model``)."""
+"""Score models.  Importing the package registers ``'ncsnpp'`` and ``'ddpm'`` (``models/utils.register_model``)."""
 from . import utils
 from . import ncsnpp
+from . import ddpm

@@ -221,9 +221,9 @@ def _kind_of_corrector(corrector):
 
 def match_pc_plan(sde, model, predictor, corrector, shape, snr, n_steps, probability_flow, continuous, eps, device):
   """Return a :class:`PcPlan` when the native engine implements this sampler, else ``None``."""
-  from .models.ncsnpp import NCSNpp
+  from .models._engine import EngineModel
   model = _unwrap(model)
-  if not isinstance(model, NCSNpp) or torch.device(device).type != 'cuda' or not torch.cuda.is_available():
+  if not isinstance(model, EngineModel) or torch.device(device).type != 'cuda' or not torch.cuda.is_available():
     return None
   if type(sde) not in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE) or not continuous:
     return None

@@ -299,7 +299,7 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
                     method='RK45', eps=1e-3, device='cuda', device_solver=None):
   """Probability-flow ODE sampler (``sampling.py:414-485``): same signature, same ``(samples, nfe)`` result.
 
-  With the engine-backed NCSN++ on a CUDA device, ``method='RK45'`` and a stock VE / VP / sub-VP SDE the solve is
+  With an engine-backed network (NCSN++ or DDPM) on a CUDA device, ``method='RK45'`` and a stock VE / VP / sub-VP SDE the solve is
   device-resident (``ode.py`` + ``csrc/ode.cu``): float64 state and Dormand-Prince stages in HBM, scipy's step-size
   controller on the host, one double read back per attempted step.  Anything else - user models or SDEs, other
   ``method`` values - runs the reference's host loop over ``scipy.integrate.solve_ivp`` (each right-hand side then
@@ -318,10 +318,11 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
     if device_solver is False or method != 'RK45' or not x.is_cuda:
       return False
     from . import native
-    from .models.ncsnpp import NCSNpp
-    ok = isinstance(native._unwrap(model), NCSNpp) and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
+    from .models._engine import EngineModel
+    ok = isinstance(native._unwrap(model), EngineModel) and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
     if device_solver and not ok:
-      raise NotImplementedError('get_ode_sampler(device_solver=True) needs the engine-backed NCSNpp and a VE/VP/sub-VP SDE')
+      raise NotImplementedError('get_ode_sampler(device_solver=True) needs an engine-backed network (NCSNpp or DDPM) and a '
+                                'VE/VP/sub-VP SDE')
     return ok
 
   def ode_sampler(model, z=None):
