@@ -151,6 +151,14 @@ typedef struct {
                                  * attn_resolutions, centered and the execution fields (precision ... no_halo); it requires
                                  * conditional = 1 and scale_by_sigma = 0, and ignores skip_rescale, progressive_input, progressive,
                                  * fir_taps / fir_kernel, naive_resample and embedding_type. */
+  int tangent;                  /* 0 (default): the forward alone.  1: the plan also carries the forward-mode tangent pass of
+                                 * b200_ncsnpp_jvp: after each op its tangent op (the same contraction on the tangent buffers
+                                 * without bias and time-embedding row, or a GroupNorm(+SiLU) / softmax tangent kernel).  Taken
+                                 * by family 1 (DDPM) and by family 0 with naive_resample = 1, progressive = 0 and
+                                 * progressive_input = 0 (the DDPM++ configs), at precision 0 or 1 with lanes <= 1; anything
+                                 * else is rejected by b200_ncsnpp_create.  A tangent plan runs attention as separate
+                                 * contractions, the skip projections as their own contraction, and keeps the few-channel
+                                 * levels on the CUDA-core kernel (op labels name the form). */
 } b200_ncsnpp_config;
 
 B200_API int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out);
@@ -173,6 +181,16 @@ B200_API int b200_ncsnpp_forward(b200_ncsnpp_t* h, const float* x_nchw, const fl
 B200_API int b200_ncsnpp_tap(b200_ncsnpp_t* h, int module_index, float* dst_nchw, long long dst_cap_elems,
                              int shape_out[4], void* stream);
 B200_API long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h);
+/* Forward plus Jacobian-vector product (engine created with tangent = 1): out = net(x), jvp_out = J_net(x) v, all NCHW
+ * [B,C,H,W].  Replaces the autograd VJP of the Hutchinson-Skilling estimator (likelihood.py:26-35): for a fixed eps,
+ * eps . (J^T eps) = eps . (J eps), so the divergence needs one forward-mode pass and no backward graph.  The engine's
+ * b200_ncsnpp_forward is not available on a tangent engine; profile_forward / profile_ops there run this pass with v = x
+ * and both results written to out. */
+B200_API int b200_ncsnpp_jvp(b200_ncsnpp_t* h, const float* x_nchw, const float* labels, int labels_uniform,
+                             const float* v_nchw, float* out_nchw, float* jvp_out_nchw, void* stream);
+/* debug (tangent = 1, keep_activations = 1): the tangent of all_modules[index]'s output, as b200_ncsnpp_tap */
+B200_API int b200_ncsnpp_tap_tangent(b200_ncsnpp_t* h, int module_index, float* dst_nchw, long long dst_cap_elems,
+                                     int shape_out[4], void* stream);
 /* One eager forward with a CUDA-event pair around every op; per-kind totals (kind 0 tensor-core
  * contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc):
  * device milliseconds, algorithmic FLOPs (2*M*N*K of the contractions) and op counts. */
@@ -246,6 +264,11 @@ B200_API int b200_ode_stage_f64(const double* y, const double* k, long long n, c
  * scalars_dev = {c_f, g2, std} */
 B200_API int b200_ode_drift_f64(const float* x32, const float* net_out, long long n, const float* scalars_dev, double* k_out,
                                 void* stream);
+/* Divergence of the drift for the likelihood ODE (likelihood.py:66-67, 95): k_out[img] (float64, the logp slots of a stage
+ * derivative) = sum_i eps_i (c_f eps_i - 0.5 g2 dscore_i), dscore = -(jvp_out / std) (std > 0) or jvp_out, with
+ * jvp_out = J_net eps from b200_ncsnpp_jvp; same scalars_dev as b200_ode_drift_f64.  Deterministic fp64 sum per image. */
+B200_API int b200_ode_div_f64(const float* eps, const float* jvp_out, int nimg, long long per_img, const float* scalars_dev,
+                              double* k_out, void* stream);
 /* ws[0] = sum_i ((h * sum_{j<nk} e[j] K[j][i]) / (atol + max(|y_i|, |y_new_i|) * rtol))^2   (RungeKutta._estimate_error_norm);
  * ws: b200_ode_workspace_doubles() doubles; deterministic two-pass reduction */
 B200_API long long b200_ode_workspace_doubles(void);

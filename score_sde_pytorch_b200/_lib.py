@@ -32,7 +32,7 @@ class NcsnppConfig(ctypes.Structure):
               ('precision', c_int), ('keep_activations', c_int), ('lanes', c_int),
               ('cuda_core_head', c_int), ('separate_groupnorm', c_int),
               ('embedding_type', c_int), ('naive_resample', c_int), ('progressive', c_int), ('pdl', c_int),
-              ('no_halo', c_int), ('family', c_int)]
+              ('no_halo', c_int), ('family', c_int), ('tangent', c_int)]
 
 
 class PcConfig(ctypes.Structure):
@@ -81,6 +81,8 @@ SIGNATURES = {
   'b200_ncsnpp_forward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
   'b200_ncsnpp_tap': (c_int, [c_void_p, c_int, c_void_p, c_ll, P(c_int), c_void_p]),
   'b200_ncsnpp_launches_per_forward': (c_ll, [c_void_p]),
+  'b200_ncsnpp_jvp': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+  'b200_ncsnpp_tap_tangent': (c_int, [c_void_p, c_int, c_void_p, c_ll, P(c_int), c_void_p]),
   'b200_ncsnpp_profile_forward': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                           P(c_float), P(ctypes.c_double), P(c_ll)]),
   'b200_pc_create': (c_int, [c_void_p, P(PcConfig), c_int, P(c_void_p)]),
@@ -92,6 +94,7 @@ SIGNATURES = {
   'b200_pc_launches_per_step': (c_ll, [c_void_p]),
   'b200_ode_stage_f64': (c_int, [c_void_p, c_void_p, c_ll, P(ctypes.c_double), c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]),
   'b200_ode_drift_f64': (c_int, [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_void_p]),
+  'b200_ode_div_f64': (c_int, [c_void_p, c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p]),
   'b200_ode_workspace_doubles': (c_ll, []),
   'b200_ode_error_sumsq_f64': (c_int, [c_void_p, c_void_p, c_void_p, c_ll, P(ctypes.c_double), c_int, ctypes.c_double,
                                        ctypes.c_double, ctypes.c_double, c_void_p, c_void_p]),

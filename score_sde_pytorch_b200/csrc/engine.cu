@@ -45,6 +45,7 @@ struct Tensor {
   float* p = nullptr; int C = 0, H = 0, W = 0; long long bytes = 0;
   double* qs = nullptr;   // GroupNorm quad sums [B][C/4][2]
   bool f16 = false;       // elements are IEEE fp16 (mid-block conv output in fp16 operand mode)
+  float* d = nullptr;     // tangent of the same shape (tangent plans: allocated right after the primal elements)
 };
 
 class Arena {
@@ -123,6 +124,7 @@ struct b200_ncsnpp {
   long long launches = 0;
   // per-call arguments read by the closures
   const float* in_x = nullptr; const float* in_labels = nullptr; float* out = nullptr; int uniform = 0;
+  const float* in_v = nullptr; float* tout = nullptr;   // b200_ncsnpp_jvp: tangent direction and J v (tangent plans)
 
   const float* W(int pi) const { return wblob + params[pi].off; }
   ~b200_ncsnpp() {
@@ -277,7 +279,8 @@ int build_graph(b200_ncsnpp* e) {
     // few tokens (T <= 64: the 4x4 block of CIFAR-10, the 8x8, 512-channel bottleneck of FFHQ-1024): one CTA per image
     // (attn_small_kernel); otherwise the block runs as separate contractions
     const bool small_ok = attn_small_supported(T, C);
-    m.tc0 = tcmode && (C % 128 == 0) && (m.tcattn || small_ok);   // q/k/v projections on tensor cores
+    m.tc0 = tcmode && (C % 128 == 0) && (m.tcattn || (small_ok && !c.tangent));   // q/k/v projections on tensor cores
+    // (tangent plans run every attention block as separate contractions: no small-token core, no fused core)
     m.gn0w = add_param(e, nm("GroupNorm_0.weight"), {C}, PK_COPY, 0, 0, 0, 0);
     m.gn0b = add_param(e, nm("GroupNorm_0.bias"), {C}, PK_COPY, 0, 0, 0, 0);
     // q,k,v projection weights packed as one [3C][C] block (rows: q, k, v), biases as one [3C] vector
@@ -404,15 +407,20 @@ struct Builder {
   int om = 1;                                  // operand store mode of tensor-core inputs: 1 TF32-grid fp32, 2 fp16
   std::string next_name;                       // label of the next op (shape summary for the per-op profile)
   double next_bytes = 0.0;                     // algorithmic HBM bytes of the next op
+  bool tan = false;                            // tangent plan (cfg.tangent): every tensor carries its tangent in Tensor::d
+  bool tan_op = false;                         // the op being added is a tangent op (labelled "tangent[...]")
   void name(const char* fmt, ...) {
     char buf[160]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap); next_name = buf;
   }
   Builder(b200_ncsnpp* e_, int B_, char* base_, bool dry_, int lane_ = 0) : e(e_), B(B_), base(base_), dry(dry_), arena(e_->cfg.keep_activations != 0), lane(lane_) {
     fused_stats = e_->cfg.precision != 1;
     om = e_->cfg.precision == 2 ? 2 : 1;
-    lowc_gn = e_->cfg.precision == 0 && e_->cfg.separate_groupnorm != 2;
+    tan = e_->cfg.tangent != 0;
+    lowc_gn = e_->cfg.precision == 0 && e_->cfg.separate_groupnorm != 2 && !tan;
     if (dry_) stats_base = reinterpret_cast<char*>(uintptr_t(1) << 40);   // any non-null base: only offsets matter in a dry run
   }
+  // the tangent of t as a tensor of its own (for the linear ops, which run the forward kernels on it)
+  static Tensor tg(const Tensor& t) { Tensor r = t; r.p = t.d; r.d = nullptr; r.qs = nullptr; return r; }
   double* qalloc(int C) {
     const long long bytes = ((long long)B * (C / 4) * 2 * 8 + 255) & ~255LL;
     double* p = reinterpret_cast<double*>(stats_base + stats_top);
@@ -421,9 +429,10 @@ struct Builder {
   }
 
   Tensor talloc(int C, int H, int W) {
-    Tensor t; t.C = C; t.H = H; t.W = W; t.bytes = (long long)B * H * W * C * 4;
+    Tensor t; t.C = C; t.H = H; t.W = W; t.bytes = (long long)B * H * W * C * 4 * (tan ? 2 : 1);
     const long long off = arena.alloc(t.bytes); arena.note();
     t.p = reinterpret_cast<float*>(base + off);
+    if (tan) t.d = t.p + (long long)B * H * W * C;
     return t;
   }
   float* falloc(long long floats, long long* bytes_out) {
@@ -431,7 +440,13 @@ struct Builder {
     const long long off = arena.alloc(*bytes_out); arena.note();
     return reinterpret_cast<float*>(base + off);
   }
-  void tfree(Tensor& t) { if (t.p) arena.release((char*)t.p - base, t.bytes); t.p = nullptr; }
+  void tfree(Tensor& t) { if (t.p) arena.release((char*)t.p - base, t.bytes); t.p = nullptr; t.d = nullptr; }
+  // a plain buffer and, in tangent plans, its tangent twin (*dp; nullptr otherwise): one allocation of twice the size
+  float* falloc2(long long floats, long long* bytes_out, float** dp) {
+    float* p = falloc(floats * (tan ? 2 : 1), bytes_out);
+    *dp = tan ? p + floats : nullptr;
+    return p;
+  }
   void ffree(float* p, long long bytes) { arena.release((char*)p - base, bytes); }
 
   // kind: 0 tensor-core contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc
@@ -439,7 +454,10 @@ struct Builder {
     if (dry) return;
     e->launches += launches;
     static const char* kind_names[] = {"tensor-core contraction", "cuda-core contraction", "groupnorm", "fir", "softmax", "time embedding", "misc", "mma.sync contraction"};
-    (lane ? e->ops2 : e->ops).push_back({kind, flops, std::move(f), next_name.empty() ? std::string(kind_names[kind & 7]) : next_name, next_bytes});
+    std::string label = next_name.empty() ? std::string(kind_names[kind & 7]) : next_name;
+    // tangent ops of a tangent plan: their own launch on the tangent buffers ("separate" form; no 2B-image contraction)
+    if (tan_op) label = "tangent[separate]: " + label;
+    (lane ? e->ops2 : e->ops).push_back({kind, flops, std::move(f), label, next_bytes});
     next_name.clear(); next_bytes = 0.0;
   }
 
@@ -453,7 +471,8 @@ struct Builder {
   }
   // GroupNorm group count: min(C/4, 32) in NCSN++ (layerspp.py:219, 235), 32 everywhere in DDPM (layers.py:562, 625, 633)
   int groups(int C) const { return e->cfg.family == 1 ? 32 : std::min(C / 4, 32); }
-  void gn(Tensor& x1, Tensor& x2, int pgw, int pgb, int act, int round, Tensor y, float* raw) {
+  // draw: tangent of the raw copy (tangent plans)
+  void gn(Tensor& x1, Tensor& x2, int pgw, int pgb, int act, int round, Tensor y, float* raw, float* draw = nullptr) {
     const int C = x1.C + x2.C, G = groups(C), HW = x1.H * x1.W;
     if ((C / G) % 4 != 0) {
       // groups that are not whole channel quads (C = 192 -> 6 channels per group): the generic two-kernel path
@@ -463,6 +482,7 @@ struct Builder {
       const Tensor a = x1, b = x2; const int Bc = B;
       name("gn_generic %d+%d @%d (%d-channel groups)", x1.C, x2.C, x1.H, C / G);
       op(3, [=](cudaStream_t st) { return launch_gn_generic(a.p, a.C, b.p, b.C, g, bt, Bc, HW, G, 1e-6f, act, round, y.p, raw, mr, st); }, 2);
+      if (tan) gn_tangent(x1, x2, g, bt, act, round, y, draw, mr, G, HW);   // reads the primal mean / rstd table
       ffree(mr, mb);
       return;
     }
@@ -473,6 +493,17 @@ struct Builder {
     op(1, [=](cudaStream_t st) {
       return launch_gn_apply(a.p, a.C, b.p, b.C, a.qs, b.qs, g, bt, Bc, HW, G, 1e-6f, act, round, y.p, raw, st, a.f16 ? 1 : 0);
     }, 2);
+    if (tan) gn_tangent(x1, x2, g, bt, act, round, y, draw, nullptr, G, HW);   // reads the primal quad sums
+  }
+  void gn_tangent(const Tensor& a, const Tensor& b, const float* g, const float* bt, int act, int round, const Tensor& y, float* draw,
+                  const float* mr, int G, int HW) {
+    const int Bc = B;
+    name("gn_tangent %d+%d @%d%s%s (%s stats)", a.C, b.C, a.H, act ? " silu" : "", draw ? " +raw" : "", mr ? "generic" : "quad");
+    tan_op = true;
+    op(1, [=](cudaStream_t st) {
+      return launch_gn_tangent(a.p, a.d, a.C, b.p, b.d, b.C, a.qs, b.qs, mr, g, bt, Bc, HW, G, 1e-6f, act, round, y.d, draw, st);
+    }, 2);
+    tan_op = false;
   }
 
   // ---- GroupNorm coefficient tables for the few-channel convolutions that normalise while staging their input ----
@@ -528,7 +559,7 @@ struct Builder {
             const float* residual, float scale, int round, Tensor& out, bool want_stats = false, int stride = 1,
             int Hin = 0, Tensor x3 = Tensor(), Tensor x4 = Tensor(), int pw2 = -1, int pb2 = -1, const Coef* gnc = nullptr) {
     Epilogue ep; memset(&ep, 0, sizeof(ep));
-    ep.bias = e->W(pb);
+    ep.bias = pb >= 0 ? e->W(pb) : nullptr;   // pb < 0: no bias (tangent ops)
     ep.rowvec = nullptr;   // patched at launch (depends on the per-call buffers)
     ep.residual = residual; ep.ld_res = Cout; ep.scale = scale; ep.round_tf32 = round;
     ep.rows_per_img = out.H * out.W; ep.out = out.p; ep.ld_out = Cout;
@@ -578,7 +609,8 @@ struct Builder {
       s.epi = ep;
       // few-channel levels of the nf = 16 networks: warp-level TF32 MMAs keep them at the HBM roofline (conv_lowc.cu);
       // strict-fp32 mode and every other shape stay on the CUDA-core kernel
-      const bool lowc = e->cfg.precision != 1 && !a1.f16 && !a2.f16 && sumC % 2 == 0 && conv_lowc_supported(s);
+      // (tangent plans keep every level on the CUDA-core kernel)
+      const bool lowc = e->cfg.precision != 1 && !tan && !a1.f16 && !a2.f16 && sumC % 2 == 0 && conv_lowc_supported(s);
       if (want_stats && lowc && fused_stats) { out.qs = qalloc(Cout); s.qstats = out.qs; }   // the epilogue sums what the next GroupNorm needs
       if (gnc) {
         if (!lowc) { set_error("ncsnpp: GroupNorm on load planned for a convolution the few-channel kernel does not take"); rc = 2; return; }
@@ -593,6 +625,17 @@ struct Builder {
         return lowc ? launch_conv_lowc(c, st) : launch_conv_simt(c, st);
       }, lowc ? 7 : 1, cflops);
     }
+  }
+
+  // tangent of conv(): the same contraction over the tangents of its operands, without bias and time-embedding row;
+  // dres: the tangent of the residual
+  void conv_t(bool use_tc, const Tensor& a1, const Tensor& a2, int taps, int pw, int Cout, const float* dres, float scale, int round,
+              const Tensor& out, int stride = 1, int Hin = 0) {
+    if (!tan) return;
+    Tensor o = tg(out);
+    tan_op = true;
+    conv(use_tc, tg(a1), tg(a2), taps, pw, -1, Cout, -1, dres, scale, round, o, /*want_stats=*/false, stride, Hin);
+    tan_op = false;
   }
 
   // batched C[b] = A[b] * W[b]^T
@@ -658,7 +701,7 @@ struct Builder {
     if (!lc0) {
       a0 = talloc(Cin, H, H);
       if (m.has_conv2 && m.tc2 && !resample) raw = talloc(Cin, H, H);
-      gn(x1, x2, m.gn0w, m.gn0b, 1, (m.tc0 && !resample) ? om : 0, a0, raw.p);
+      gn(x1, x2, m.gn0w, m.gn0b, 1, (m.tc0 && !resample) ? om : 0, a0, raw.p, raw.d);
     }
     Tensor xr;
     if (resample) {
@@ -668,6 +711,12 @@ struct Builder {
       xr.f16 = m.tc2 && om == 2;
       resample2x(a0.p, H, Cin, m.up != 0, m.tc0 ? om : 0, a0r.p);
       resample2x(x1.p, H, Cin, m.up != 0, m.tc2 ? om : 0, xr.p);
+      if (tan) {   // the resampling is linear: the same kernels on the tangents
+        tan_op = true;
+        resample2x(a0.d, H, Cin, m.up != 0, m.tc0 ? om : 0, a0r.d);
+        resample2x(x1.d, H, Cin, m.up != 0, m.tc2 ? om : 0, xr.d);
+        tan_op = false;
+      }
       tfree(a0); a0 = a0r;
     }
     Tensor h1 = talloc(m.cout, Ho, Ho);
@@ -680,6 +729,7 @@ struct Builder {
       ffree(c0.scale, c0.bytes);
     } else {
       conv(m.tc0, a0, Tensor(), 9, m.c0w, m.c0b, m.cout, m.dense_row, nullptr, 1.f, h1_f16 ? 2 : 0, h1, /*want_stats=*/true);
+      conv_t(m.tc0, a0, Tensor(), 9, m.c0w, m.cout, nullptr, 1.f, 0, h1);
       tfree(a0);
     }
     if (h1_f16 && !h1.qs) { set_error("ncsnpp: fp16 mid-block tensor without fused GroupNorm sums"); rc = 2; return Tensor(); }
@@ -693,9 +743,11 @@ struct Builder {
     }
     Tensor s;
     const float* residual = x1.p;
+    const float* dresidual = x1.d;
     // Fused skip projection (default): Conv_2(x) (layerspp.py:270) is accumulated inside the second 3x3 convolution
-    // as extra K steps instead of a separate launch + a residual round trip through HBM.
-    if (m.has_conv2 && m.tc1 && m.tc2 && (resample || raw.p)) {
+    // as extra K steps instead of a separate launch + a residual round trip through HBM.  (Tangent plans: its bias rides
+    // in the row-vector slot, so the skip projection stays a contraction of its own there.)
+    if (m.has_conv2 && m.tc1 && m.tc2 && (resample || raw.p) && !tan) {
       Tensor out = talloc(m.cout, Ho, Ho);
       Tensor e1 = resample ? xr : raw, e2 = Tensor();
       e1.f16 = false;   // conv() addresses operands by the engine-wide operand mode
@@ -705,11 +757,15 @@ struct Builder {
     }
     if (m.has_conv2) {
       s = talloc(m.cout, Ho, Ho);
-      if (resample) conv(m.tc2, xr, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-      else if (m.tc2 && raw.p) conv(true, raw, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-      else if (m.tc2) conv(true, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-      else conv(false, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-      residual = s.p;
+      if (resample) { conv(m.tc2, xr, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
+                      conv_t(m.tc2, xr, Tensor(), 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
+      else if (m.tc2 && raw.p) { conv(true, raw, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
+                                 conv_t(true, raw, Tensor(), 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
+      else if (m.tc2) { conv(true, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
+                        conv_t(true, x1, x2, 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
+      else { conv(false, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
+             conv_t(false, x1, x2, 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
+      residual = s.p; dresidual = s.d;
       tfree(raw); tfree(xr);
     } else if (x2.p) { set_error("ncsnpp: concat input without a skip convolution"); rc = 2; return Tensor(); }
     Tensor out = talloc(m.cout, Ho, Ho);
@@ -718,6 +774,7 @@ struct Builder {
       ffree(c1.scale, c1.bytes); tfree(h1);
     } else {
       conv(m.tc1, a1, Tensor(), 9, m.c1w, m.c1b, m.cout, -1, residual, inv_s2, 0, out, /*want_stats=*/true);
+      conv_t(m.tc1, a1, Tensor(), 9, m.c1w, m.cout, dresidual, inv_s2, 0, out);
       tfree(a1);
     }
     tfree(s);
@@ -741,6 +798,7 @@ struct Builder {
     Tensor a = talloc(C, x.H, x.W);
     gn(x, none, m.gn0w, m.gn0b, 0, (tc || small) ? om : 0, a, nullptr);
     long long ob; float* O = nullptr;
+    float* dO = nullptr;   // tangent of O (tangent plans)
     if (small) {
       long long qb; float* qkv = falloc(BT * 3 * C, &qb);
       // q | k | v = a [Wq; Wk; Wv]^T + [bq; bk; bv]   (layerspp.py:78-80) as one N=3C contraction
@@ -754,19 +812,26 @@ struct Builder {
       ffree(qkv, qb);
     } else {
       long long qkb, vtb, sb;
-      float* qk = falloc((long long)B * T * 2 * C, &qkb);
-      float* vT = falloc((long long)B * C * T, &vtb);
+      float *dqk = nullptr, *dvT = nullptr, *dS = nullptr;   // tangents (tangent plans)
+      float* qk = falloc2((long long)B * T * 2 * C, &qkb, &dqk);
+      float* vT = falloc2((long long)B * C * T, &vtb, &dvT);
       // q,k = a Wq^T + bq | a Wk^T + bk   (layerspp.py:78-79) in one N=2C contraction
       gemm(tc, a.p, C, BT, 0 /* rows enumerated flat */, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, bqkv, nullptr, 0, 1.f, tc ? om : 0, qk, 2 * C);
       // v^T[b][c][t] = sum_i Wv[c][i] a[b][t][i]   (bias bv is added after the PV product: softmax rows sum to 1)
       gemm(tc, wv, C, C, 0, a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, vT, T, nullptr, 1 << 30);
+      if (tan) {   // dq, dk, dv: the projections of da, without bias
+        tan_op = true;
+        gemm(tc, a.d, C, BT, 0, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, dqk, 2 * C);
+        gemm(tc, wv, C, C, 0, a.d, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, dvT, T, nullptr, 1 << 30);
+        tan_op = false;
+      }
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
       // [T,T] logits/probabilities and the attention output stay on chip; other token counts (tf32 mode) use separate launches.
       if (om == 2 && !(tc && m.tc2 && tc_attn_supported(T, C))) {
         set_error("ncsnpp: fp16 operand mode needs the fused attention core (T=%d C=%d)", T, C); rc = 2; return Tensor();
       }
-      if (tc && m.tc2 && tc_attn_supported(T, C)) {
+      if (tc && m.tc2 && tc_attn_supported(T, C) && !tan) {
         Tensor out = talloc(C, x.H, x.W);
         if (fused_stats) out.qs = qalloc(C);
         if (!dry) {
@@ -783,20 +848,43 @@ struct Builder {
         ffree(qk, qkb); ffree(vT, vtb);
         return out;
       }
-      float* S = falloc(BT * T, &sb);
+      float* S = falloc2(BT * T, &sb, &dS);
       // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax
       gemm(tc, qk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30);
+      if (tan) {   // dS = dq k^T + q dk^T
+        long long tb; float* t1 = falloc(BT * T, &tb);
+        tan_op = true;
+        gemm(tc, dqk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, t1, T, nullptr, 1 << 30);
+        gemm(tc, qk, 2 * C, BT, T, dqk + C, 2 * C, BT, T, B, T, T, C, nullptr, t1, T, 1.f, 0, dS, T, nullptr, 1 << 30);
+        tan_op = false;
+        ffree(t1, tb);
+      }
       ffree(qk, qkb);
       name("softmax T=%d", T);
       op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
-      O = falloc(BT * C, &ob);
+      if (tan) {   // dP = P (sc dS - rowsum(P sc dS)), over dS
+        name("softmax_tangent T=%d", T);
+        tan_op = true;
+        op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
+        tan_op = false;
+      }
+      O = falloc2(BT * C, &ob, &dO);
       // h[b][q][c] = sum_k P[q][k] v[k][c] + bv[c]   (layerspp.py:86)
       gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? 1 : 0, O, C);
+      if (tan) {   // dO = dP v + P dv
+        long long tb; float* t2 = falloc(BT * C, &tb);
+        tan_op = true;
+        gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
+        gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? 1 : 0, dO, C);
+        tan_op = false;
+        ffree(t2, tb);
+      }
       ffree(S, sb); ffree(vT, vtb);
     }
     Tensor out = talloc(C, x.H, x.W);
-    Tensor Ot; Ot.p = O; Ot.C = C; Ot.H = x.H; Ot.W = x.W;
+    Tensor Ot; Ot.p = O; Ot.C = C; Ot.H = x.H; Ot.W = x.W; Ot.d = dO;
     conv(m.tc2, Ot, Tensor(), 1, m.nw[3], m.nb[3], C, -1, x.p, inv_s2, 0, out, /*want_stats=*/true);   // NIN_3 + (x+h)/sqrt2 (:87-91)
+    conv_t(m.tc2, Ot, Tensor(), 1, m.nw[3], C, x.d, inv_s2, 0, out);
     ffree(O, ob);
     return out;
   }
@@ -814,7 +902,15 @@ struct Builder {
       name("operand copy %d @%d", x.C, H);
       next_bytes = (double)n * (4.0 + (om == 2 ? 2.0 : 4.0));
       op(1, [=](cudaStream_t st) { return launch_store_operand(src, dst, n, omc, st); }, 6);
+      if (tan) {
+        const float* dsrc = x.d; float* ddst = xo.d;
+        name("operand copy %d @%d", x.C, H);
+        tan_op = true;
+        op(1, [=](cudaStream_t st) { return launch_store_operand(dsrc, ddst, n, omc, st); }, 6);
+        tan_op = false;
+      }
       conv(true, xo, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true, /*stride=*/2, /*Hin=*/H);
+      conv_t(true, xo, Tensor(), 9, m.w, m.cout, nullptr, 1.f, 0, out, /*stride=*/2, /*Hin=*/H);
       tfree(xo);
     } else {
       SimtConv s; memset(&s, 0, sizeof(s));
@@ -823,6 +919,13 @@ struct Builder {
       s.epi.bias = e->W(m.b); s.epi.scale = 1.f; s.epi.rows_per_img = Ho * Ho; s.epi.out = out.p; s.epi.ld_out = m.cout;
       name("conv3x3 s2 %d->%d @%d [cuda-core]", x.C, m.cout, Ho);
       op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
+      if (tan) {
+        SimtConv sd = s; sd.x1 = x.d; sd.epi.bias = nullptr; sd.epi.out = out.d;
+        name("conv3x3 s2 %d->%d @%d [cuda-core]", x.C, m.cout, Ho);
+        tan_op = true;
+        op(1, [=](cudaStream_t st) { return launch_conv_simt(sd, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
+        tan_op = false;
+      }
     }
     return out;
   }
@@ -833,8 +936,10 @@ struct Builder {
     const int H = x.H, Ho = 2 * H;
     Tensor u = talloc(x.C, Ho, Ho);
     fir(x.p, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, u.p, 1.f, /*box=*/true);
+    if (tan) { tan_op = true; fir(x.d, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, u.d, 1.f, /*box=*/true); tan_op = false; }
     Tensor out = talloc(m.cout, Ho, Ho);
     conv(m.tc0, u, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true);
+    conv_t(m.tc0, u, Tensor(), 9, m.w, m.cout, nullptr, 1.f, 0, out);
     tfree(u);
     return out;
   }
@@ -866,7 +971,8 @@ struct Builder {
       }, 5);
     }
     // ---- input (ncsnpp.py:259-268) ----
-    float* xc = falloc((long long)B * ch * R * R, &xcb);   // 2x-1 when data is not centred; NCHW
+    float* dxc = nullptr;   // its tangent: v, or 2v (tangent plans)
+    float* xc = falloc2((long long)B * ch * R * R, &xcb, &dxc);   // 2x-1 when data is not centred; NCHW
     {
       const long long n = (long long)B * ch * R * R;
       const int centered = c.centered;
@@ -875,6 +981,15 @@ struct Builder {
         launch_kernel(affine_kernel, dim3((int)std::min<long long>((n + 255) / 256, 4096)), dim3(256), 0, st, eng->in_x_l[ln], xc, n, -0.5f, 2.0f);
         return cudaGetLastError() == cudaSuccess ? 0 : (set_error("affine launch failed"), 1);
       });
+      if (tan) {
+        tan_op = true;
+        op(1, [=](cudaStream_t st) {
+          if (centered) return cudaMemcpyAsync(dxc, eng->in_v, n * 4, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : (set_error("memcpy failed"), 1);
+          launch_kernel(affine_kernel, dim3((int)std::min<long long>((n + 255) / 256, 4096)), dim3(256), 0, st, eng->in_v, dxc, n, 0.0f, 2.0f);
+          return cudaGetLastError() == cudaSuccess ? 0 : (set_error("affine launch failed"), 1);
+        });
+        tan_op = false;
+      }
     }
     size_t mi = 3;
     std::vector<Tensor> hs;
@@ -884,12 +999,21 @@ struct Builder {
       if (m.tc0 || m.tc1) {
         // im2col patches [B*R*R][32] (TF32 grid) then one K=32 contraction with the flat-packed weights (tensor cores, or the
         // few-channel kernel for nf <= 64)
-        long long pb; float* patches = falloc((long long)B * R * R * 32, &pb);   // 128 B per pixel: 32 fp32 or 64 fp16
+        float* dpatches = nullptr;
+        long long pb; float* patches = falloc2((long long)B * R * R * 32, &pb, &dpatches);   // 128 B per pixel: 32 fp32 or 64 fp16
         const int Bc = B, omc = om;
         name("im2col 3x3 %d @%d", ch, R);
         op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(xc, patches, Bc, ch, R, R, R, R, 1, 1, omc, st); }, 6);
+        if (tan) {
+          name("im2col 3x3 %d @%d", ch, R);
+          tan_op = true;
+          op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(dxc, dpatches, Bc, ch, R, R, R, R, 1, 1, omc, st); }, 6);
+          tan_op = false;
+        }
         Tensor pt; pt.p = patches; pt.C = om == 2 ? 64 : 32; pt.H = R; pt.W = R;   // patches as a one-K-step NHWC image: a 1x1 conv
+        pt.d = dpatches;
         conv(m.tc0, pt, Tensor(), 1, m.w, m.b, nf, -1, nullptr, 1.f, 0, h0, /*want_stats=*/true);
+        conv_t(m.tc0, pt, Tensor(), 1, m.w, nf, nullptr, 1.f, 0, h0);
         ffree(patches, pb);
       } else {
         SimtConv s; memset(&s, 0, sizeof(s));
@@ -897,6 +1021,12 @@ struct Builder {
         s.OH = R; s.OW = R; s.nbatch = B; s.a_batched = 1; s.w = e->W(m.w); s.N = nf;
         s.epi.bias = e->W(m.b); s.epi.scale = 1.f; s.epi.rows_per_img = R * R; s.epi.out = h0.p; s.epi.ld_out = nf;
         op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * R * R * (double)nf * ch * 9);
+        if (tan) {
+          SimtConv sd = s; sd.x1 = dxc; sd.epi.bias = nullptr; sd.epi.out = h0.d;
+          tan_op = true;
+          op(1, [=](cudaStream_t st) { return launch_conv_simt(sd, st); }, 1, 2.0 * B * R * R * (double)nf * ch * 9);
+          tan_op = false;
+        }
       }
       hs.push_back(h0);
       tap(m.index, h0);
@@ -1067,6 +1197,19 @@ struct Builder {
             tc_gemm_set_head(pl, eng->out_l[ln], sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1);
             return tc_gemm_launch(pl, st);
           }, 0, 2.0 * B * R * R * (double)ch * a.C * 9);
+          if (tan) {   // J v: the same head over the tangent, without bias, into the jvp output
+            TcGemmDesc dd = d; dd.a1 = a.d; dd.epi.bias = nullptr;
+            TcGemmPlan* pt = nullptr;
+            if (int r = tc_gemm_plan_create(dd, &pt)) { rc = r; return r; }
+            e->tcplans.push_back(pt);
+            name("conv3x3 %d->%d(pad 128) @%d nchw-out /sigma [%s]", a.C, ch, R, tc_gemm_form(pt));
+            tan_op = true;
+            op(1, [=](cudaStream_t st) {
+              tc_gemm_set_head(pt, eng->tout, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1);
+              return tc_gemm_launch(pt, st);
+            }, 0, 2.0 * B * R * R * (double)ch * a.C * 9);
+            tan_op = false;
+          }
         }
       } else if (ch <= 4) {
         name("conv3x3 %d->%d @%d nchw-out [small-n]", a.C, ch, R);
@@ -1074,6 +1217,15 @@ struct Builder {
           return launch_conv3x3_small_n(ain.p, wo, bo, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1, eng->out_l[ln],
                                         Bc, R, R, ain.C, ch, head_f16, st);
         }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
+        if (tan) {
+          name("conv3x3 %d->%d @%d nchw-out [small-n]", a.C, ch, R);
+          tan_op = true;
+          op(1, [=](cudaStream_t st) {
+            return launch_conv3x3_small_n(ain.d, wo, nullptr, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1, eng->tout,
+                                          Bc, R, R, ain.C, ch, head_f16, st);
+          }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
+          tan_op = false;
+        }
       } else {
         SimtConv s; memset(&s, 0, sizeof(s));
         s.x1 = a.p; s.C1 = a.C; s.in_scale = 1.f; s.H = R; s.W = R; s.R = s.S = 3; s.stride = 1; s.pad = 1;
@@ -1085,6 +1237,17 @@ struct Builder {
           if (sbs) { cc.epi.per_img_div = eng->in_labels_l[ln]; cc.epi.div_stride = eng->uniform ? 0 : 1; }
           return launch_conv_simt(cc, st);
         }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
+        if (tan) {
+          SimtConv sd = s; sd.x1 = a.d; sd.epi.bias = nullptr;
+          tan_op = true;
+          op(1, [=](cudaStream_t st) {
+            SimtConv cc = sd;
+            cc.epi.out = eng->tout;
+            if (sbs) { cc.epi.per_img_div = eng->in_labels_l[ln]; cc.epi.div_stride = eng->uniform ? 0 : 1; }
+            return launch_conv_simt(cc, st);
+          }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
+          tan_op = false;
+        }
       }
       tfree(a);
     }
@@ -1125,6 +1288,21 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
                  "without time conditioning, models/ddpm.py:58-71)");
     B200_REQUIRE(!cfg->scale_by_sigma, "ncsnpp_create: DDPM (family 1) with scale_by_sigma = 1 (configs/ve/cifar10_ddpm.py) is not "
                  "supported by the engine");
+  }
+  if (cfg->tangent) {
+    // the forward-mode tangent pass (b200_ncsnpp_jvp) covers DDPM and the DDPM++ family; everything else is refused here
+    // rather than approximated
+    B200_REQUIRE(cfg->tangent == 1, "ncsnpp_create: tangent=%d unknown (0 or 1)", cfg->tangent);
+    B200_REQUIRE(cfg->precision == 0 || cfg->precision == 1, "ncsnpp_create: tangent = 1 with precision = %d: the tangent pass "
+                 "runs in precision 0 (tf32) or 1 (fp32), not on fp16 operands", cfg->precision);
+    B200_REQUIRE(cfg->lanes <= 1, "ncsnpp_create: tangent = 1 with lanes = %d: the tangent pass runs one lane", cfg->lanes);
+    if (cfg->family == 0) {
+      B200_REQUIRE(cfg->naive_resample, "ncsnpp_create: tangent = 1 with naive_resample = 0: FIR resampling has no tangent pass");
+      B200_REQUIRE(cfg->progressive == 0, "ncsnpp_create: tangent = 1 with progressive = %d: the output_skip pyramid has no "
+                   "tangent pass", cfg->progressive);
+      B200_REQUIRE(cfg->progressive_input == 0, "ncsnpp_create: tangent = 1 with progressive_input = %d: the input pyramid has "
+                   "no tangent pass", cfg->progressive_input);
+    }
   }
   b200_ncsnpp* e = new b200_ncsnpp();
   e->cfg = *cfg;
@@ -1254,6 +1432,7 @@ void set_call_args(b200_ncsnpp* h, const float* x, const float* labels, int unif
 int b200_ncsnpp_forward(b200_ncsnpp_t* h, const float* x, const float* labels, int uniform, float* out, void* stream) {
   B200_REQUIRE(h && x && labels && out, "forward: null argument");
   B200_REQUIRE(!h->ops.empty(), "forward: no plan bound (call b200_ncsnpp_bind_workspace)");
+  B200_REQUIRE(!h->cfg.tangent, "forward: the engine was created with tangent = 1; call b200_ncsnpp_jvp");
   PdlScope pdl(h->cfg.pdl != 0);            // launches of this call carry the programmatic-dependent-launch attribute
   set_call_args(h, x, labels, uniform, out);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1279,11 +1458,25 @@ int b200_ncsnpp_forward(b200_ncsnpp_t* h, const float* x, const float* labels, i
   return 0;
 }
 
+int b200_ncsnpp_jvp(b200_ncsnpp_t* h, const float* x, const float* labels, int uniform, const float* v, float* out, float* jvp_out,
+                    void* stream) {
+  B200_REQUIRE(h && x && labels && v && out && jvp_out, "jvp: null argument");
+  B200_REQUIRE(h->cfg.tangent, "jvp: the engine was not created with tangent = 1");
+  B200_REQUIRE(!h->ops.empty(), "jvp: no plan bound (call b200_ncsnpp_bind_workspace)");
+  PdlScope pdl(h->cfg.pdl != 0);
+  set_call_args(h, x, labels, uniform, out);
+  h->in_v = v; h->tout = jvp_out;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (auto& o : h->ops) if (int r = o.fn(st)) return r;   // one lane (b200_ncsnpp_create rejects lanes = 2 with tangent = 1)
+  return 0;
+}
+
 int b200_ncsnpp_profile_forward(b200_ncsnpp_t* h, const float* x, const float* labels, int uniform, float* out,
                                 void* stream, float ms_by_kind[8], double flops_by_kind[8], long long ops_by_kind[8]) {
   B200_REQUIRE(h && x && labels && out && ms_by_kind, "profile_forward: null argument");
   B200_REQUIRE(!h->ops.empty(), "profile_forward: no plan bound");
   set_call_args(h, x, labels, uniform, out);
+  h->in_v = x; h->tout = out;   // tangent plans: the JVP pass along v = x
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   for (int k = 0; k < 8; ++k) { ms_by_kind[k] = 0.f; if (flops_by_kind) flops_by_kind[k] = 0.0; if (ops_by_kind) ops_by_kind[k] = 0; }
   // both lanes serially on ONE stream: each launch is timed alone (no overlap), which is what a per-kernel roofline needs
@@ -1337,6 +1530,7 @@ int b200_ncsnpp_profile_ops(b200_ncsnpp_t* h, const float* x, const float* label
   const long long n = (long long)(h->ops.size() + h->ops2.size());
   B200_REQUIRE(cap >= n, "profile_ops: need room for %lld ops", n);
   set_call_args(h, x, labels, uniform, out);
+  h->in_v = x; h->tout = out;   // tangent plans: the JVP pass along v = x
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   std::vector<cudaEvent_t> ev(n + 1);
   for (auto& e : ev) B200_CHECK_CUDA(cudaEventCreate(&e));
@@ -1361,6 +1555,17 @@ int b200_ncsnpp_tap(b200_ncsnpp_t* h, int module_index, float* dst, long long ca
   if (shape_out) { shape_out[0] = h->B; shape_out[1] = t.C; shape_out[2] = t.H; shape_out[3] = t.W; }
   B200_REQUIRE(cap >= n, "tap: destination too small (%lld < %lld)", cap, n);
   return launch_nhwc_to_nchw(t.p, dst, h->B, t.H * t.W, t.C, static_cast<cudaStream_t>(stream));
+}
+
+int b200_ncsnpp_tap_tangent(b200_ncsnpp_t* h, int module_index, float* dst, long long cap, int shape_out[4], void* stream) {
+  B200_REQUIRE(h && h->cfg.keep_activations && h->cfg.tangent, "tap_tangent: engine was not created with keep_activations=1, tangent=1");
+  auto it = h->taps.find(module_index);
+  B200_REQUIRE(it != h->taps.end() && it->second.d, "tap_tangent: module %d has no recorded tangent", module_index);
+  const Tensor& t = it->second;
+  const long long n = (long long)h->B * t.C * t.H * t.W;
+  if (shape_out) { shape_out[0] = h->B; shape_out[1] = t.C; shape_out[2] = t.H; shape_out[3] = t.W; }
+  B200_REQUIRE(cap >= n, "tap_tangent: destination too small (%lld < %lld)", cap, n);
+  return launch_nhwc_to_nchw(t.d, dst, h->B, t.H * t.W, t.C, static_cast<cudaStream_t>(stream));
 }
 
 long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h) { return h ? h->launches : 0; }

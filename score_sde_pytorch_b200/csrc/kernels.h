@@ -46,6 +46,16 @@ int launch_conv3x3_small_n(const float* x, const float* w, const float* bias, co
                            float* out_nchw, int B, int H, int W, int C, int N, int x_f16, cudaStream_t st,
                            const float* add_nchw = nullptr);
 
+// ---- tangent.cu : forward-mode tangents of the nonlinear ops (b200_ncsnpp_jvp) --------------------------------------
+// GroupNorm(+SiLU) tangent of a (two-source) NHWC tensor: x = primal input, d = its tangent; the primal statistics come from
+// the quad sums q1/q2 or, for groups that are not channel quads, the generic path's mean / rstd table mr (float2 per
+// (image, group)).  dy (and draw, the tangent of the input in operand format, optional) are stored in mode round_out (0, 1).
+int launch_gn_tangent(const float* x1, const float* d1, int C1, const float* x2, const float* d2, int C2, const double* q1,
+                      const double* q2, const float* mr, const float* gamma, const float* beta, int B, int HW, int G, float eps,
+                      int act, int round_out, float* dy, float* draw, cudaStream_t st);
+// dP = P (scale dS - rowsum(P scale dS)) over rows of length T, written over ds
+int launch_softmax_tangent(const float* p, float* ds, long long rows, int T, float scale, int round_out, cudaStream_t st);
+
 // ---- conv_simt.cu : strict-fp32 CUDA-core implicit GEMM (any shape) ---------
 struct SimtConv {
   // A operand

@@ -50,6 +50,27 @@ __global__ void __launch_bounds__(ODE_THREADS) ode_drift_kernel(const float* __r
   }
 }
 
+// k_out[img] = sum_i eps_i * (J_drift eps)_i with (J_drift eps) = c_f * eps - (g2 * dscore) * 0.5, dscore the score's
+// tangent (-(jvp / std) for VP / sub-VP, jvp for VE) in the drift kernel's fp32 operation order; one CTA per image,
+// fixed-order fp64 reduction
+__device__ __forceinline__ void block_sum_to(double v, double* dst);
+__global__ void __launch_bounds__(ODE_THREADS) ode_div_kernel(const float* __restrict__ eps, const float* __restrict__ jvp,
+                                                              long long per_img, const float* __restrict__ scal,
+                                                              double* __restrict__ k_out) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  const float c_f = scal[0], g2 = scal[1], sd = scal[2];
+  const long long base = (long long)blockIdx.x * per_img;
+  double s = 0.0;
+  for (long long i = threadIdx.x; i < per_img; i += blockDim.x) {
+    const float e = eps[base + i];
+    float ds = jvp[base + i];
+    if (sd > 0.f) ds = -__fdiv_rn(ds, sd);
+    const float jd = __fsub_rn(__fmul_rn(c_f, e), __fmul_rn(__fmul_rn(g2, ds), 0.5f));
+    s += (double)e * (double)jd;
+  }
+  block_sum_to(s, k_out + blockIdx.x);
+}
+
 __device__ __forceinline__ void block_sum_to(double v, double* dst) {
   __shared__ double sh[ODE_THREADS / 32];
   v = warp_sum_d(v);
@@ -120,6 +141,15 @@ int b200_ode_stage_f64(const double* y, const double* k, long long n, const doub
 int b200_ode_drift_f64(const float* x32, const float* net_out, long long n, const float* scalars_dev, double* k_out, void* stream) {
   B200_REQUIRE(x32 && net_out && scalars_dev && k_out && n > 0, "ode_drift: null argument");
   launch_kernel(ode_drift_kernel, dim3(ode_grid(n)), dim3(ODE_THREADS), 0, static_cast<cudaStream_t>(stream), x32, net_out, n, scalars_dev, k_out);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+int b200_ode_div_f64(const float* eps, const float* jvp_out, int nimg, long long per_img, const float* scalars_dev,
+                     double* k_out, void* stream) {
+  B200_REQUIRE(eps && jvp_out && scalars_dev && k_out && nimg > 0 && per_img > 0, "ode_div: bad argument");
+  launch_kernel(ode_div_kernel, dim3(nimg), dim3(ODE_THREADS), 0, static_cast<cudaStream_t>(stream), eps, jvp_out, per_img,
+                scalars_dev, k_out);
   B200_CHECK_LAUNCH();
   return 0;
 }

@@ -58,6 +58,7 @@ class EngineModel(nn.Module):
   def _init_engine(self):
     """Call once ``all_modules`` is complete."""
     self._engine = None        # (handle, blob, workspace, batch, weights_version)
+    self._tan_engine = None    # the same for the tangent-enabled engine of jvp(), created on first use
     self._weights_version = 0
     self._link_parameters()    # lets models.ema.ExponentialMovingAverage tell this module to repack
     # fires for direct loads and for loads through a wrapper (DataParallel(model).load_state_dict calls
@@ -130,12 +131,32 @@ class EngineModel(nn.Module):
     return super().load_state_dict(sd, strict=strict, **kw)   # the post hook invalidates the packed weights
 
   def _release(self):
-    """Destroy the native engine.  Every cached PC plan holds a pointer to it, so they are released first."""
+    """Destroy the native engines.  Every cached PC plan holds a pointer to the primal one, so they are released first."""
     for plan in self.__dict__.get('_pc_plans', {}).values():
       plan._release()
     if self.__dict__.get('_engine') is not None:
       _lib.load().b200_ncsnpp_destroy(self._engine['h'])
       self._engine = None
+    self._release_tangent()
+
+  def _release_tangent(self):
+    if self.__dict__.get('_tan_engine') is not None:
+      _lib.load().b200_ncsnpp_destroy(self._tan_engine['h'])
+      self._tan_engine = None
+
+  def check_jvp_supported(self):
+    """Raise ``NotImplementedError`` naming the field if this configuration has no forward-mode tangent pass (``jvp``).
+    Creates and destroys a tangent-enabled engine handle; needs no GPU."""
+    name = type(self).__name__
+    if self.precision == 'f16':
+      raise NotImplementedError(f"{name}.jvp: precision='f16' has no tangent pass; use precision='tf32' or 'fp32'")
+    cfg = self._native_config()
+    cfg.tangent = 1
+    h = ctypes.c_void_p()
+    lib = _lib.load()
+    if lib.b200_ncsnpp_create(ctypes.byref(cfg), ctypes.byref(h)) != 0:
+      raise NotImplementedError(f'{name}.jvp: {_lib.last_error()}')
+    lib.b200_ncsnpp_destroy(h)
 
   @staticmethod
   def _explicit_device(device):
@@ -152,26 +173,36 @@ class EngineModel(nn.Module):
     except Exception:
       pass
 
-  def engine(self, batch, device):
+  def engine(self, batch, device, tangent=False):
     """Create / re-plan the native engine for ``batch`` images on ``device``.  ``eng['gen']`` is a monotonically
     increasing plan generation: it changes whenever the engine, its workspace or its plan is rebuilt, which is what
-    dependants (captured CUDA graphs in ``native.PcPlan``) key their validity on."""
+    dependants (captured CUDA graphs in ``native.PcPlan``) key their validity on.
+
+    ``tangent=True``: the separate tangent-enabled engine of :meth:`jvp` (``b200_ncsnpp_config.tangent = 1``), with its own
+    weights and workspace; the primal engine, its PC plans and the generation counter are not touched."""
     device = self._explicit_device(device)
-    eng = self._engine
+    eng = self._tan_engine if tangent else self._engine
     if eng is not None and (eng['device'] != device or eng['precision'] != self.precision):
-      self._release()
+      self._release_tangent() if tangent else self._release()
       eng = None
     if eng is None:
       h = ctypes.c_void_p()
       cfg = self._native_config()
+      if tangent:
+        self.check_jvp_supported()
+        cfg.tangent = 1
       _lib.call('b200_ncsnpp_create', ctypes.byref(cfg), ctypes.byref(h))
       nbytes = _lib.load().b200_ncsnpp_weights_bytes(h)
       blob = torch.zeros(nbytes // 4 + 64, dtype=torch.float32, device=device)
       _lib.call('b200_ncsnpp_bind_weights', h, _lib.ptr(blob))
-      self._generation = getattr(self, '_generation', 0) + 1
+      if not tangent:
+        self._generation = getattr(self, '_generation', 0) + 1
       eng = dict(h=h, blob=blob, ws=None, batch=0, wver=-1, device=device, precision=self.precision,
-                 table=self._param_table(h), gen=self._generation)
-      self._engine = eng
+                 table=self._param_table(h), gen=None if tangent else self._generation)
+      if tangent:
+        self._tan_engine = eng
+      else:
+        self._engine = eng
     if eng['wver'] != self._weights_version:
       sd = dict(self.named_parameters())
       pos_freqs = getattr(self, 'pos_freqs', None)   # the sinusoidal embedding's frequency table (a pseudo-parameter)
@@ -195,8 +226,9 @@ class EngineModel(nn.Module):
         eng['ws'] = torch.empty(need // 4 + 256, dtype=torch.float32, device=device)
       _lib.call('b200_ncsnpp_bind_workspace', eng['h'], batch, _lib.ptr(eng['ws']), eng['ws'].numel() * 4)
       eng['batch'] = batch
-      self._generation += 1
-      eng['gen'] = self._generation
+      if not tangent:
+        self._generation += 1
+        eng['gen'] = self._generation
     return eng
 
   def forward(self, x, time_cond, labels_uniform=False):
@@ -217,6 +249,43 @@ class EngineModel(nn.Module):
       _lib.call('b200_ncsnpp_forward', eng['h'], _lib.ptr(xin), _lib.ptr(lab), int(bool(labels_uniform)),
                 _lib.ptr(out), _lib.stream_ptr(x.device))
     return out
+
+  def jvp(self, x, time_cond, v, labels_uniform=False):
+    """``(net(x), J_net(x) v)`` in one forward-mode pass of the tangent-enabled engine (``b200_ncsnpp_jvp``): the
+    Jacobian-vector product the likelihood's divergence needs (``likelihood.py:26-35``), without autograd.  Configurations
+    without a tangent pass raise ``NotImplementedError`` (:meth:`check_jvp_supported`)."""
+    name = type(self).__name__
+    if not x.is_cuda:
+      raise RuntimeError(f'{name}.jvp runs on CUDA devices only')
+    if x.dim() != 4 or x.shape[1] != self.config.data.num_channels or x.shape[2] != self.config.data.image_size \
+        or x.shape[3] != self.config.data.image_size:
+      raise RuntimeError(f'{name}: input shape {tuple(x.shape)} does not match the configured image geometry')
+    if tuple(v.shape) != tuple(x.shape):
+      raise RuntimeError(f'{name}.jvp: tangent shape {tuple(v.shape)} differs from the input shape {tuple(x.shape)}')
+    with torch.cuda.device(x.device):
+      eng = self.engine(x.shape[0], x.device, tangent=True)
+      xin = x.detach().to(torch.float32).contiguous()
+      vin = v.detach().to(device=x.device, dtype=torch.float32).contiguous()
+      lab = time_cond.detach().to(device=x.device, dtype=torch.float32).contiguous()
+      if lab.numel() != x.shape[0]:
+        raise RuntimeError(f'{name}: time_cond has {lab.numel()} entries for a batch of {x.shape[0]}')
+      out = torch.empty_like(xin)
+      jv = torch.empty_like(xin)
+      _lib.call('b200_ncsnpp_jvp', eng['h'], _lib.ptr(xin), _lib.ptr(lab), int(bool(labels_uniform)), _lib.ptr(vin),
+                _lib.ptr(out), _lib.ptr(jv), _lib.stream_ptr(x.device))
+    return out, jv
+
+  def tap_tangent(self, module_index):
+    """Debug (``keep_activations=True``, after :meth:`jvp`): the tangent of ``all_modules[module_index]``'s output, NCHW."""
+    eng = self._tan_engine
+    if eng is None:
+      raise RuntimeError('tap_tangent: run jvp first')
+    shape = (ctypes.c_int * 4)()
+    buf = torch.empty(min(1 << 28, eng['ws'].numel()), dtype=torch.float32, device=eng['device'])
+    _lib.call('b200_ncsnpp_tap_tangent', eng['h'], module_index, _lib.ptr(buf), buf.numel(), shape,
+              _lib.stream_ptr(eng['device']))
+    n = shape[0] * shape[1] * shape[2] * shape[3]
+    return buf[:n].reshape(shape[0], shape[1], shape[2], shape[3]).clone()
 
   def activation_range_report(self, x, time_cond, limit=65504.0):
     """Largest magnitude of every module output of one evaluation, measured with an fp32-range (`'tf32'`) copy of this
@@ -254,11 +323,13 @@ class EngineModel(nn.Module):
   def launches_per_forward(self):
     return int(_lib.load().b200_ncsnpp_launches_per_forward(self._engine['h'])) if self._engine else 0
 
-  def op_names(self):
-    """Shape labels of the ops of the bound plan, in execution order (b200_ncsnpp_op_info); empty before the first call."""
-    if not self._engine:
+  def op_names(self, tangent=False):
+    """Shape labels of the ops of the bound plan, in execution order (b200_ncsnpp_op_info); empty before the first call.
+    ``tangent=True``: the plan of the tangent-enabled engine of :meth:`jvp`."""
+    eng = self._tan_engine if tangent else self._engine
+    if not eng:
       return []
-    h = self._engine['h']
+    h = eng['h']
     n = int(_lib.load().b200_ncsnpp_num_ops(h))
     buf, kind, fl = ctypes.create_string_buffer(200), ctypes.c_int(), ctypes.c_double()
     names = []

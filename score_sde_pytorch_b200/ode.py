@@ -126,16 +126,24 @@ class DormandPrince45:
 
 class CudaOdeOps:
   """The float64 state ``y`` / ``y_new``, the stage derivatives ``K[7][n]`` and the float32 network input on the device.
-  ``drift(t, x32, k_out)`` (given by the sampler) evaluates the network on ``x32`` and writes the float64 drift."""
+  ``drift(t, x32, k_out)`` (given by the sampler) evaluates the network on ``x32`` and writes the float64 drift.
 
-  def __init__(self, x0, drift):
+  ``extra`` > 0 appends that many zero-initialised float64 entries to the state (the likelihood ODE's ``logp`` slots,
+  ``likelihood.py:98``): ``x32`` is then the image part of the float32 stage state and ``k_out`` the whole stage row."""
+
+  def __init__(self, x0, drift, extra=0):
     self.device = x0.device
     self.shape = tuple(x0.shape)
-    self.n = x0.numel()
-    self.y = x0.detach().to(torch.float64).reshape(-1).contiguous()
+    self.n_img = x0.numel()
+    y = x0.detach().to(torch.float64).reshape(-1)
+    if extra:
+      y = torch.cat([y, torch.zeros(extra, dtype=torch.float64, device=self.device)])
+    self.n = y.numel()
+    self.y = y.contiguous()
     self.y_new = torch.empty_like(self.y)
     self.K = torch.empty(N_STAGES + 1, self.n, dtype=torch.float64, device=self.device)
-    self.x32 = torch.empty(self.shape, dtype=torch.float32, device=self.device)
+    self.x32_flat = torch.empty(self.n, dtype=torch.float32, device=self.device)
+    self.x32 = self.x32_flat[:self.n_img].view(self.shape)
     self.ws = torch.zeros(int(_lib.load().b200_ode_workspace_doubles()), dtype=torch.float64, device=self.device)
     self.drift = drift
     self.host_reads = 0
@@ -149,7 +157,7 @@ class CudaOdeOps:
   def rhs(self, t, coefs, h, slot, keep_y):
     st = _lib.stream_ptr(self.device)
     _lib.call('b200_ode_stage_f64', _lib.ptr(self.y), _lib.ptr(self.K), self.n, self._coefs(coefs), len(coefs), float(h),
-              _lib.ptr(self.y_new) if keep_y else None, _lib.ptr(self.x32), st)
+              _lib.ptr(self.y_new) if keep_y else None, _lib.ptr(self.x32_flat), st)
     self.drift(t, self.x32, self.K[slot])
 
   def _read(self):
@@ -173,7 +181,11 @@ class CudaOdeOps:
     self.K[0].copy_(self.K[N_STAGES])         # FSAL: self.f = f_new
 
   def state_f32(self):
-    return self.y.to(torch.float32).reshape(self.shape)
+    return self.y[:self.n_img].to(torch.float32).reshape(self.shape)
+
+  def extra_state(self):
+    """The appended float64 entries of the state (``extra`` > 0)."""
+    return self.y[self.n_img:].clone()
 
 
 def engine_drift_fn(sde, model, batch, device):
@@ -204,3 +216,38 @@ def engine_drift_fn(sde, model, batch, device):
               _lib.stream_ptr(device))
 
   return drift
+
+
+def engine_likelihood_fn(sde, model, epsilon):
+  """Right-hand side of the likelihood ODE (``likelihood.py:91-96``) over the augmented state ``[x; logp]`` for the
+  engine-backed network: one ``b200_ncsnpp_jvp`` evaluation gives the network output and ``J_net eps``; the drift goes to
+  ``k_out[:n]`` (``b200_ode_drift_f64``, as the ODE sampler) and the per-image divergence ``eps . (J_drift eps)`` to the
+  logp slots ``k_out[n:]`` (``b200_ode_div_f64``).  Scalars as in :func:`engine_drift_fn`."""
+  from . import sde_lib
+  vp_like = isinstance(sde, (sde_lib.VPSDE, sde_lib.subVPSDE))
+  device = epsilon.device
+  batch = epsilon.shape[0]
+  n = epsilon.numel()
+  eps = epsilon.contiguous()
+  one = torch.ones(1, 1, 1, 1, device=device)
+  zero = torch.zeros(1, 1, 1, 1, device=device)
+  scal = torch.zeros(3, dtype=torch.float32, device=device)
+
+  def rhs(t, x32, k_out):
+    vec_t = torch.ones(1, device=device) * t
+    f1, g = sde.sde(one, vec_t)
+    std = sde.marginal_prob(zero, vec_t)[1]
+    if vp_like:
+      labels = vec_t * 999
+      scal[2:3] = std
+    else:
+      labels = std
+      scal[2] = 0.0
+    scal[0:1] = f1.reshape(1)
+    scal[1:2] = g ** 2
+    out, jv = model.jvp(x32, labels.to(torch.float32).expand(batch).contiguous(), eps, labels_uniform=True)
+    st = _lib.stream_ptr(device)
+    _lib.call('b200_ode_drift_f64', _lib.ptr(x32), _lib.ptr(out), n, _lib.ptr(scal), _lib.ptr(k_out), st)
+    _lib.call('b200_ode_div_f64', _lib.ptr(eps), _lib.ptr(jv), batch, n // batch, _lib.ptr(scal), _lib.ptr(k_out[n:]), st)
+
+  return rhs
