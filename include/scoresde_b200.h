@@ -136,13 +136,12 @@ typedef struct {
   int pdl;                      /* 1: every launch of a forward / PC iteration carries the programmatic-dependent-launch attribute
                                  * (each kernel waits for its predecessor with griddepcontrol.wait after its own prologue, so launch
                                  * latency and barrier init of kernel k+1 overlap the tail of kernel k) */
-  int no_halo;                  /* (the Python host sets 2 unless told otherwise.)  0 or 2: swapped-form 3x3 convolutions (128 output channels) on
+  int no_halo;                  /* (the Python host sets 2 unless told otherwise.)  0 or 2: swapped-form 3x3 'same' convolutions on
                                  * 16- / 32-pixel-wide images read three W-shifted halo copies of their tile per channel chunk (csrc/gemm_tc.cu
                                  * "halo form": 2.4x fewer L2 -> shared-memory bytes than one shifted tile per filter tap); 1: one shifted
                                  * tile per tap everywhere (kept for A/B); + 4: with an L2 prefetch of the next tile's halo boxes; + 8:
-                                 * row-major launches of shapes with a halo form walk K in that form's order, so plans of different batch
-                                 * sizes agree bit for bit (tests).  Swapped-form results are bit-identical in every mode (same products,
-                                 * same order). */
+                                 * accepted and ignored (it used to make row-major launches walk K in the halo form's order, which every
+                                 * launch of such a shape now does).  Results are bit-identical in every mode (same products, same order). */
   int family;                   /* 0 = NCSN++ / DDPM++ (models/ncsnpp.py, the default); 1 = DDPM (models/ddpm.py:39-181): ResnetBlockDDPM
                                  * with the NIN_0 skip (layers.py:619-662), AttnBlock (:558-581), Downsample / Upsample with_conv
                                  * (:584-616), residual scale 1, GroupNorm with 32 groups everywhere (channel counts must be multiples

@@ -10,7 +10,8 @@
 //
 // Kernels (persistent, warp-specialised, 384 threads):
 //   gemm_tc_kernel<BN>   one CTA per tile: 128 rows x BN columns, or - `swap` - 128 output channels x 256 pixels
-//                        (D^T = W X^T) for 128-channel convolutions, 1x1 convolutions and the network head;
+//                        (D^T = W X^T) for 128-channel convolutions, 1x1 convolutions, the network head and the 3x3
+//                        'same' convolutions on 16- / 32-pixel rows (any output width: one tile per 128-channel slice);
 //   attn_tc_kernel<F16>  attn_tc.cuh: QK^T, softmax, PV, NIN_3 + residual in one kernel.
 // Roles: warp 0 TMA producer (4-D box of the NHWC tensor shifted by the filter tap - or, in the halo form, three
 // W-shifted copies of the tile with its halo per channel chunk - zero halo and tail rows from out-of-bounds fill,
@@ -511,8 +512,8 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
         const int ntaps = src < 2 ? p.taps : 1;
         // K order.  Default: filter tap, then channel chunk - consecutive loads sweep the channel vector of the same shifted
         // pixels (contiguous 128-byte segments of every pixel row).  Shapes that have a halo form (p.chunk_major) walk K the way that form must -
-        // channel chunk, filter column, filter row - so that halo on / off add the same products in the same order and
-        // are bit-identical (the nine-load loop of such a shape only runs in A/B checks).
+        // channel chunk, filter column, filter row - so that halo on / off and row-major launches of such shapes add
+        // the same products in the same order.
         const int nouter = p.chunk_major ? nch : ntaps, ninner = p.chunk_major ? ntaps : nch;
         for (int o = 0; o < nouter; ++o) {
           for (int i = 0; i < ninner; ++i) {
@@ -656,11 +657,19 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     //  * swapped operands (D^T = W X^T: 128 output channels x 256 pixels per tile) for 128-channel outputs, whose
     //    M=128,N=128 MMAs are issue-bound, and for 1x1 convolutions (output-bound launches: the swapped form's
     //    epilogue writes whole channel vectors of a pixel); the NCHW head exists only in this form;
+    //  * 3x3 'same' filters on 16- / 32-pixel rows with more output channels take the swapped form too, as tiles_n
+    //    128-channel halves of each 256-pixel tile: it has the halo form (about 29 KB brought into shared memory per
+    //    K step of a 128 x 256 tile instead of 48 KB).  It has as many tiles as the row-major plan, except below ~34
+    //    images at 16x16 (~9 at 32x32), where the row-major plan would split into 128-column tiles; those small launches
+    //    stay swapped all the same, because a swapped tile's wgmma sums are not bitwise those of a row-major tile, and
+    //    every batch size should compute each output as the large-batch plan does;
     //  * launches too small to give every SM a 256-column tile are cut into 128-column tiles: twice the CTAs at work.
     const long long Mtot = (long long)d.nimg * d.H * d.W;
     // (image rows wider than 128 pixels - the 256..1024-pixel families - are cut into 128-pixel boxes like any other: the
     // two boxes of a 256-pixel tile are then two halves of one row or of consecutive rows)
-    const bool can_swap = d.conv && p.stride == 1 && (d.N_total % 256 != 0 || d.taps == 1) && (d.H * d.W) % 256 == 0 &&
+    const bool halo_geom = d.taps == 9 && p.pad == 1 && (d.W == 16 || d.W == 32) && (d.Hin == 0 || d.Hin == d.H) &&
+                           (d.Win == 0 || d.Win == d.W);
+    const bool can_swap = d.conv && p.stride == 1 && (d.N_total % 256 != 0 || d.taps == 1 || halo_geom) && (d.H * d.W) % 256 == 0 &&
                           (d.W <= BM || d.W % BM == 0) && Mtot % 256 == 0 && d.epi.rows_per_img % 256 == 0;
     p.swap = can_swap ? 1 : 0;
     if (d.epi.out_nchw && !p.swap) { delete pl; B200_REQUIRE(false, "gemm_tc: the NCHW head needs the swapped-operand form"); }
@@ -720,12 +729,12 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     const int tile_px = p.swap ? 256 : BM;
     const bool halo = (d.no_halo & 3) != 1 && d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && p.swap &&
                       (d.W == 16 || d.W == 32) && (d.H * d.W) % tile_px == 0 && (d.Hin == 0 || d.Hin == d.H) && (d.Win == 0 || d.Win == d.W);
-    // swapped-form shapes that have a halo form keep its K order when it is switched off (bit-identical A/B).  `no_halo & 8`
-    // asks the same of row-major launches of such shapes, so that plans of different batch sizes add the same products in
-    // the same order (plan-agreement tests)
+    // every launch of a shape that has a halo form walks K in that form's order, swapped or row-major, halo on or off: the
+    // A/B of the two mainloops is bit-identical, and a row-major launch of such a shape (one the swapped form does not
+    // take) adds the same products in the same order
     const bool halo_shape = d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && (d.W == 16 || d.W == 32) && (d.H * d.W) % tile_px == 0 &&
                             (d.Hin == 0 || d.Hin == d.H) && (d.Win == 0 || d.Win == d.W);
-    p.chunk_major = (halo_shape && (p.swap || (d.no_halo & 8))) ? 1 : 0;
+    p.chunk_major = halo_shape ? 1 : 0;
     if (halo) {
       const int rows = tile_px / d.W;
       p.halo = 1; p.halo_dh_bytes = d.W * 128; p.halo_copy_bytes = (rows + 2) * d.W * 128;

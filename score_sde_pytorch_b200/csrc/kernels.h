@@ -115,7 +115,7 @@ struct TcGemmDesc {
   int no_halo;              // halo form of the 3x3 mainloop (three W-shifted halo copies per channel chunk instead of nine shifted
                             // tiles): 0 or 2 = in the swapped form, 1 = never;
                             // + 4 = with an L2 prefetch (UTMAPF) of the next tile's halo boxes (A/B: measured 2 % slower);
-                            // + 8 = single-CTA row-major launches of shapes the pair kernel runs in halo form walk K in that form's order
+                            // + 8 = accepted, no effect (every launch of a shape with a halo form walks K in that form's order)
   double* qstats;           // optional GroupNorm quad sums [img][N_total/4][2] accumulated by the epilogue (mode 1)
   Epilogue epi;
 };
