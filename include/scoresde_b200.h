@@ -230,6 +230,16 @@ typedef struct {
   float snr;
   const float *label, *score_scale, *alpha, *pa, *pb, *pc;   /* HOST tables [n_steps] */
   const float *ca, *cb, *cc;   /* HOST tables [n_steps] of the affine corrector (corrector == 2), else NULL */
+  /* controllable generation (controllable_generation.py:8-198): after the corrector block and again after the predictor
+   * block (even a None one) the state is blended with a fresh draw from the data marginal, in the latent space
+   * y = decouple(x):  y' = y*(1-mask) + (cm*known + cs*z)*mask,  x = couple(y'),
+   * x_mean = couple(decouple(x)*(1-mask) + cm*known*mask).  Each blend draws one randn_like(x). */
+  int constraint;              /* 0 off, 1 inpaint (decouple = identity), 2 colorize (decouple(v)_j = sum_i v_i color_m[3i+j]) */
+  const float *cm, *cs;        /* HOST tables [n_steps]: mean coefficient and std of sde.marginal_prob at t_i */
+  float color_m[9], color_minv[9];   /* colorize: M and M^-1, row-major */
+  int noise_nhwc;              /* 1: every randn_like draw fills the state in channels-last memory order, as torch does for
+                                * a channels-last x (the reference's colorization state is its einsum's channels-last
+                                * output for batches > 1); 0: NCHW order */
 } b200_pc_config;
 
 B200_API int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b200_pc_t** out);
@@ -243,7 +253,11 @@ B200_API int b200_pc_bind_workspace(b200_pc_t* pc, void* ws_dev, long long ws_by
 B200_API int b200_pc_run(b200_pc_t* pc, float* x, float* x_mean, int first_step, int num_steps,
                          unsigned long long seed, unsigned long long offset, unsigned long long* offset_out,
                          int use_graph, void* stream);
-/* One iteration with caller-supplied noise tensors (NCHW, may be NULL when unused). */
+/* Constrained plans: the blend's `known` (the data; for colorization already decouple(gray)) and `mask`, both full
+ * NCHW device tensors of the batch shape.  Rebinding other pointers re-captures the graph on the next run.
+ * `stream` matches b200_pc_bind_workspace's signature; nothing is enqueued on it. */
+B200_API int b200_pc_bind_constraint(b200_pc_t* pc, const float* known, const float* mask, void* stream);
+/* One iteration with caller-supplied noise tensors (NCHW, may be NULL when unused).  Not for constrained plans. */
 B200_API int b200_pc_step_external(b200_pc_t* pc, float* x, float* x_mean, int step,
                                    const float* noise_corrector, const float* noise_predictor, void* stream);
 B200_API long long b200_pc_launches_per_step(const b200_pc_t* pc);

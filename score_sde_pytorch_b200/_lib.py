@@ -41,7 +41,9 @@ class PcConfig(ctypes.Structure):
               ('snr', c_float),
               ('label', P(c_float)), ('score_scale', P(c_float)), ('alpha', P(c_float)),
               ('pa', P(c_float)), ('pb', P(c_float)), ('pc', P(c_float)),
-              ('ca', P(c_float)), ('cb', P(c_float)), ('cc', P(c_float))]
+              ('ca', P(c_float)), ('cb', P(c_float)), ('cc', P(c_float)),
+              ('constraint', c_int), ('cm', P(c_float)), ('cs', P(c_float)),
+              ('color_m', c_float * 9), ('color_minv', c_float * 9), ('noise_nhwc', c_int)]
 
 
 # name -> (restype, argtypes); must list every symbol declared in include/scoresde_b200.h
@@ -90,6 +92,7 @@ SIGNATURES = {
   'b200_pc_workspace_bytes': (c_ll, [c_void_p]),
   'b200_pc_bind_workspace': (c_int, [c_void_p, c_void_p, c_ll, c_void_p]),
   'b200_pc_run': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_ull, c_ull, P(c_ull), c_int, c_void_p]),
+  'b200_pc_bind_constraint': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
   'b200_pc_step_external': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
   'b200_pc_launches_per_step': (c_ll, [c_void_p]),
   'b200_ode_stage_f64': (c_int, [c_void_p, c_void_p, c_ll, P(ctypes.c_double), c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]),

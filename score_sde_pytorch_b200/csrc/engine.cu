@@ -1577,12 +1577,16 @@ long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h) { return h ? 
 // ===========================================================================
 struct b200_pc {
   b200_ncsnpp* model; b200_pc_config cfg; int B; long long numel, per_img;
-  std::vector<float> h_label, h_ss, h_alpha, h_pa, h_pb, h_pc, h_ca, h_cb, h_cc;
+  std::vector<float> h_label, h_ss, h_alpha, h_pa, h_pb, h_pc, h_ca, h_cb, h_cc, h_cm, h_cs;
   // workspace carve-up
   char* ws = nullptr; float *d_label, *d_ss, *d_alpha, *d_pa, *d_pb, *d_pc, *d_ca, *d_cb, *d_cc, *labels, *net_out, *norms, *means;
+  float *d_cm = nullptr, *d_cs = nullptr;
   int* d_step; unsigned long long* d_offset;
   PhiloxMap map;
+  const float* known = nullptr; const float* mask = nullptr;   // constrained plans: bound by b200_pc_bind_constraint
+  PcColorTransform color{};
   cudaGraphExec_t gexec = nullptr; float* graph_x = nullptr; float* graph_xm = nullptr; cudaStream_t graph_stream = nullptr;
+  const float* graph_known = nullptr; const float* graph_mask = nullptr;
   unsigned long long graph_seed = 0;
   cudaStream_t cap_stream = nullptr;   // the legacy default stream cannot be captured: capture on a private one
   long long launches_per_step = 0;
@@ -1601,7 +1605,20 @@ long long pc_ws_layout(b200_pc* pc, char* base) {
   pc->labels = (float*)take(pc->B * 4LL); pc->net_out = (float*)take(pc->numel * 4LL);
   pc->norms = (float*)take(2LL * pc->B * 4); pc->means = (float*)take(256);
   pc->d_step = (int*)take(256); pc->d_offset = (unsigned long long*)take(256);
+  if (pc->cfg.constraint) { pc->d_cm = (float*)take(N * 4LL); pc->d_cs = (float*)take(N * 4LL); }
   return off;
+}
+
+// randn_like calls per iteration: the corrector's inner steps, the predictor, and the two constraint blends
+unsigned long long pc_calls_per_step(const b200_pc_config& c) {
+  return (unsigned long long)((c.corrector ? c.n_corrector_steps : 0) + (c.predictor ? 1 : 0) + (c.constraint ? 2 : 0));
+}
+
+int pc_constrain(b200_pc* pc, float* x, float* x_mean, unsigned long long cps, unsigned long long call, cudaStream_t st) {
+  const b200_ncsnpp_config& mc = pc->model->cfg;
+  return launch_pc_constrain(x, x_mean, pc->known, pc->mask, pc->map, pc->d_offset, pc->d_step, cps, call, pc->d_cm,
+                             pc->d_cs, pc->color, pc->cfg.constraint == 2, mc.num_channels,
+                             (long long)mc.image_size * mc.image_size, st);
 }
 
 // one PC iteration at step *d_step; noise_c/noise_p non-null -> external noise
@@ -1609,7 +1626,7 @@ int pc_iteration(b200_pc* pc, float* x, float* x_mean, const float* noise_c, con
   b200_ncsnpp* m = pc->model;
   const b200_pc_config& c = pc->cfg;
   PcStepScalars sc{pc->d_ss, pc->d_alpha, pc->d_pa, pc->d_pb, pc->d_pc};
-  const unsigned long long cps = (unsigned long long)((c.corrector ? c.n_corrector_steps : 0) + (c.predictor ? 1 : 0));
+  const unsigned long long cps = pc_calls_per_step(c);
   if (int r = launch_fill_from_table(pc->d_label, pc->d_step, pc->labels, pc->B, st)) return r;
   unsigned long long call = 0;
   if (c.corrector == 2) {
@@ -1631,12 +1648,21 @@ int pc_iteration(b200_pc* pc, float* x, float* x_mean, const float* noise_c, con
       ++call;
     }
   }
+  if (c.constraint) {
+    // controllable_generation.py:43-52 / :137-146 after the corrector update, which a NoneCorrector makes the identity
+    if (int r = pc_constrain(pc, x, x_mean, cps, call, st)) return r;
+    ++call;
+  }
   if (c.predictor) {
     if (int r = b200_ncsnpp_forward(m, x, pc->labels, 1, pc->net_out, st)) return r;
     if (int r = launch_predictor_apply(x, x_mean, pc->net_out, noise_p, pc->map, pc->d_offset, pc->d_step, cps, call,
                                        sc, 1, st)) return r;
+    ++call;
   }
-  if (!c.predictor && x_mean) {
+  if (c.constraint) {
+    // the blend after the predictor writes this iteration's x_mean, also for a NonePredictor
+    if (int r = pc_constrain(pc, x, x_mean, cps, call, st)) return r;
+  } else if (!c.predictor && x_mean) {
     // NonePredictor.update_fn returns (x, x) (sampling.py:241-250): the "mean" handed to the denoise step of
     // pc_sampler (:409) is the noisy state after the corrector, not the last Langevin mean
     B200_CHECK_CUDA(cudaMemcpyAsync(x_mean, x, (size_t)pc->numel * 4, cudaMemcpyDeviceToDevice, st));
@@ -1655,6 +1681,11 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   B200_REQUIRE(cfg->corrector >= 0 && cfg->corrector <= 2, "pc_create: corrector %d unsupported", cfg->corrector);
   B200_REQUIRE(cfg->corrector != 2 || (cfg->ca && cfg->cb && cfg->cc), "pc_create: affine corrector without its tables");
   B200_REQUIRE(cfg->predictor == 0 || cfg->predictor == 1, "pc_create: predictor %d unsupported", cfg->predictor);
+  B200_REQUIRE(cfg->constraint >= 0 && cfg->constraint <= 2, "pc_create: constraint %d unsupported", cfg->constraint);
+  B200_REQUIRE(!cfg->constraint || (cfg->cm && cfg->cs), "pc_create: constraint without its cm/cs tables");
+  B200_REQUIRE(cfg->noise_nhwc == 0 || cfg->noise_nhwc == 1, "pc_create: noise_nhwc %d unsupported", cfg->noise_nhwc);
+  B200_REQUIRE(cfg->constraint != 2 || model->cfg.num_channels == 3,
+               "pc_create: colorization needs 3 channels, the model has %d", model->cfg.num_channels);
   b200_pc* pc = new b200_pc();
   pc->model = model; pc->cfg = *cfg; pc->B = batch;
   const b200_ncsnpp_config& mc = model->cfg;
@@ -1667,9 +1698,17 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   cp(pc->h_ca, cfg->ca, 1.f); cp(pc->h_cb, cfg->cb, 0.f); cp(pc->h_cc, cfg->cc, 0.f);
   pc->cfg.label = pc->cfg.score_scale = pc->cfg.alpha = pc->cfg.pa = pc->cfg.pb = pc->cfg.pc = nullptr;
   pc->cfg.ca = pc->cfg.cb = pc->cfg.cc = nullptr;
-  const long long cps = (cfg->corrector ? cfg->n_corrector_steps : 0) + (cfg->predictor ? 1 : 0);
+  if (cfg->constraint) {
+    cp(pc->h_cm, cfg->cm, 1.f); cp(pc->h_cs, cfg->cs, 0.f);
+    memcpy(pc->color.M, cfg->color_m, sizeof(pc->color.M));
+    memcpy(pc->color.Minv, cfg->color_minv, sizeof(pc->color.Minv));
+  }
+  pc->cfg.cm = pc->cfg.cs = nullptr;
+  const long long cps = (cfg->corrector ? cfg->n_corrector_steps : 0) + (cfg->predictor ? 1 : 0);   // network evaluations
+  const long long tail = cfg->constraint ? (cfg->predictor ? 1 : 0) + 2   /* predictor apply, two blends */
+                                         : 1 /* predictor apply, or the x -> x_mean copy */;
   pc->launches_per_step = cps * model->launches + (cfg->corrector == 1 ? cfg->n_corrector_steps * 3 : cfg->corrector == 2 ? cfg->n_corrector_steps : 0) +
-                          1 /* predictor apply, or the x -> x_mean copy */ + 2;
+                          tail + 2;
   *out = pc;
   return 0;
 }
@@ -1699,9 +1738,16 @@ int b200_pc_bind_workspace(b200_pc_t* pc, void* ws, long long bytes, void* strea
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_ca, pc->h_ca.data(), N * 4, cudaMemcpyHostToDevice, st));
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cb, pc->h_cb.data(), N * 4, cudaMemcpyHostToDevice, st));
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cc, pc->h_cc.data(), N * 4, cudaMemcpyHostToDevice, st));
+  if (pc->cfg.constraint) {
+    B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cm, pc->h_cm.data(), N * 4, cudaMemcpyHostToDevice, st));
+    B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cs, pc->h_cs.data(), N * 4, cudaMemcpyHostToDevice, st));
+  }
   B200_CHECK_CUDA(cudaStreamSynchronize(st));
   if (pc->gexec) { cudaGraphExecDestroy(pc->gexec); pc->gexec = nullptr; }
-  return philox_map_init(&pc->map, pc->numel, 0);
+  if (int r = philox_map_init(&pc->map, pc->numel, 0)) return r;
+  const b200_ncsnpp_config& mc = pc->model->cfg;
+  pc->map.nhwc = pc->cfg.noise_nhwc; pc->map.C = mc.num_channels; pc->map.HW = (long long)mc.image_size * mc.image_size;
+  return 0;
 }
 
 int b200_pc_run(b200_pc_t* pc, float* x, float* x_mean, int first_step, int num_steps, unsigned long long seed,
@@ -1710,16 +1756,19 @@ int b200_pc_run(b200_pc_t* pc, float* x, float* x_mean, int first_step, int num_
   PdlScope pdl(pc->model->cfg.pdl != 0);
   B200_REQUIRE(first_step >= 0 && num_steps >= 0 && first_step + num_steps <= pc->cfg.n_steps,
                "pc_run: steps [%d,%d) outside the %d-step schedule", first_step, first_step + num_steps, pc->cfg.n_steps);
+  B200_REQUIRE(!pc->cfg.constraint || (pc->known && pc->mask), "pc_run: constrained plan without b200_pc_bind_constraint");
+  B200_REQUIRE(!pc->cfg.constraint || x_mean, "pc_run: a constrained plan needs x_mean");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   pc->map.seed = seed;
   // the noise offset of step s is *d_offset + (s*cps + call)*inc, so rebase for first_step
-  const unsigned long long cps = (unsigned long long)((pc->cfg.corrector ? pc->cfg.n_corrector_steps : 0) + (pc->cfg.predictor ? 1 : 0));
+  const unsigned long long cps = pc_calls_per_step(pc->cfg);
   const unsigned long long base = offset - (unsigned long long)first_step * cps * pc->map.inc;
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_offset, &base, 8, cudaMemcpyHostToDevice, st));
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_step, &first_step, 4, cudaMemcpyHostToDevice, st));
   B200_CHECK_CUDA(cudaStreamSynchronize(st));   // host sources above are stack variables
   if (use_graph && num_steps > 0) {
-    if (!pc->gexec || pc->graph_x != x || pc->graph_xm != x_mean || pc->graph_seed != seed || pc->graph_stream != st) {
+    if (!pc->gexec || pc->graph_x != x || pc->graph_xm != x_mean || pc->graph_seed != seed || pc->graph_stream != st ||
+        pc->graph_known != pc->known || pc->graph_mask != pc->mask) {
       if (pc->gexec) { cudaGraphExecDestroy(pc->gexec); pc->gexec = nullptr; }
       cudaGraph_t g = nullptr;
       if (!pc->cap_stream) B200_CHECK_CUDA(cudaStreamCreateWithFlags(&pc->cap_stream, cudaStreamNonBlocking));
@@ -1731,6 +1780,7 @@ int b200_pc_run(b200_pc_t* pc, float* x, float* x_mean, int first_step, int num_
       B200_CHECK_CUDA(cudaGraphInstantiate(&pc->gexec, g, 0));
       cudaGraphDestroy(g);
       pc->graph_x = x; pc->graph_xm = x_mean; pc->graph_stream = st; pc->graph_seed = seed;
+      pc->graph_known = pc->known; pc->graph_mask = pc->mask;
     }
     for (int i = 0; i < num_steps; ++i) B200_CHECK_CUDA(cudaGraphLaunch(pc->gexec, st));
   } else {
@@ -1740,9 +1790,19 @@ int b200_pc_run(b200_pc_t* pc, float* x, float* x_mean, int first_step, int num_
   return 0;
 }
 
+int b200_pc_bind_constraint(b200_pc_t* pc, const float* known, const float* mask, void* stream) {
+  (void)stream;
+  B200_REQUIRE(pc && known && mask, "pc_bind_constraint: null argument");
+  B200_REQUIRE(pc->cfg.constraint, "pc_bind_constraint: the plan was created with constraint = 0");
+  pc->known = known; pc->mask = mask;   // a changed pointer re-captures the graph on the next b200_pc_run
+  return 0;
+}
+
 int b200_pc_step_external(b200_pc_t* pc, float* x, float* x_mean, int step, const float* noise_c,
                           const float* noise_p, void* stream) {
   B200_REQUIRE(pc && pc->ws && x, "pc_step_external: not bound");
+  B200_REQUIRE(!pc->cfg.constraint, "pc_step_external: not available for constrained (inpainting / colorization) plans; "
+               "use b200_pc_run");
   PdlScope pdl(pc->model->cfg.pdl != 0);
   B200_REQUIRE(step >= 0 && step < pc->cfg.n_steps, "pc_step_external: step %d out of range", step);
   B200_REQUIRE(!pc->cfg.corrector || noise_c, "pc_step_external: corrector noise missing");

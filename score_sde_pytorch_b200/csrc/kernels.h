@@ -151,6 +151,10 @@ struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` el
   long long numel;
   int grid, block;          // torch's grid/block => thread stride for element ownership
   unsigned long long inc;   // Philox offset consumed per randn call
+  // torch draws a dense tensor in memory order: with nhwc = 1 the state is channels-last (C x HW images), so draw p
+  // lands on the NCHW element of memory position p.  philox_map_init sets nhwc = 0 (contiguous NCHW).
+  int nhwc, C;
+  long long HW;
 };
 int philox_map_init(PhiloxMap* m, long long numel, unsigned long long seed);
 int launch_randn_torch(const PhiloxMap& m, const unsigned long long* offset_dev, unsigned long long offset_add,
@@ -173,6 +177,16 @@ int launch_predictor_apply(float* x, float* x_mean, const float* out, const floa
                            const unsigned long long* offset_dev, const int* step,
                            unsigned long long calls_per_step, unsigned long long call_idx,
                            PcStepScalars sc, int add_noise, cudaStream_t st);
+struct PcColorTransform {    // decouple(v)_j = sum_i v_i M[i*3+j]; couple uses Minv the same way
+  float M[9], Minv[9];
+};
+// controllable generation's data-consistency blend (inpainting: colorize = 0, no channel transform); cm/cs are the
+// device tables of the data marginal's mean coefficient and std, z is the randn_like draw at call `call_idx`
+int launch_pc_constrain(float* x, float* x_mean, const float* known, const float* mask, const PhiloxMap& m,
+                        const unsigned long long* offset_dev, const int* step,
+                        unsigned long long calls_per_step, unsigned long long call_idx,
+                        const float* cm, const float* cs, const PcColorTransform& ct, int colorize, int C, long long HW,
+                        cudaStream_t st);
 int launch_step_increment(int* step, cudaStream_t st);
 
 }  // namespace b200

@@ -29,6 +29,7 @@ int philox_map_init(PhiloxMap* m, long long numel, unsigned long long seed) {
   if (grid < 1) grid = 1;
   m->seed = seed; m->numel = numel; m->grid = (int)grid; m->block = block;
   m->inc = (unsigned long long)((numel - 1) / ((long long)block * grid * 4) + 1) * 4;
+  m->nhwc = 0; m->C = 1; m->HW = 1;
   return 0;
 }
 
@@ -48,7 +49,21 @@ __device__ __forceinline__ unsigned long long step_offset(const unsigned long lo
   return *offset_dev + (s * calls_per_step + call_idx) * inc;
 }
 
-// noise value of flat element e under torch's layout (4x redundant Philox; used only by the norm pass)
+// NCHW element that receives draw p (the draw's position in memory), and its inverse
+__device__ __forceinline__ long long draw_elem(const PhiloxMap& m, long long p) {
+  if (!m.nhwc) return p;
+  const long long chw = m.C * m.HW, b = p / chw, r = p - b * chw, hw = r / m.C;
+  return b * chw + (r - hw * m.C) * m.HW + hw;
+}
+
+__device__ __forceinline__ long long draw_index(const PhiloxMap& m, long long e) {
+  if (!m.nhwc) return e;
+  const long long chw = m.C * m.HW, b = e / chw, r = e - b * chw, c = r / m.HW;
+  return b * chw + (r - c * m.HW) * m.C + c;
+}
+
+// noise value of draw e under torch's layout (4x redundant Philox; used by the norm pass and the constraint blend,
+// whose per-pixel threads need channels that torch's layout hands to different threads)
 __device__ __forceinline__ float noise_at(const PhiloxMap& m, unsigned long long off, long long e) {
   const long long T = (long long)m.grid * m.block;
   const long long l = e / (4 * T), r = e % (4 * T);
@@ -88,7 +103,7 @@ __global__ void __launch_bounds__(256) pc_norms_kernel(const float* __restrict__
   for (int j = threadIdx.x; j < per_img; j += blockDim.x) {
     const long long e = (long long)b * per_img + j;
     const float o = out[e];
-    const float z = noise ? noise[e] : noise_at(m, off, e);
+    const float z = noise ? noise[e] : noise_at(m, off, draw_index(m, e));
     so += (double)o * o;
     sz += (double)z * z;
   }
@@ -154,12 +169,76 @@ __global__ void __launch_bounds__(256) pc_apply_kernel(float* __restrict__ x, fl
     }
 #pragma unroll
     for (int ii = 0; ii < 4; ++ii) {
-      const long long e = t + T * ii + 4 * T * l;
-      if (e >= m.numel) continue;
+      const long long p = t + T * ii + 4 * T * l;
+      if (p >= m.numel) continue;
+      const long long e = draw_elem(m, p);
       const float zz = (add_noise && noise) ? noise[e] : z[ii];
       const float xm = ca * x[e] + cb * out[e];
       if (x_mean) x_mean[e] = xm;
       x[e] = add_noise ? xm + cz * zz : xm;
+    }
+  }
+}
+
+// Data-consistency step of controllable generation (controllable_generation.py:43-52 inpainting, :137-146 colorization),
+// one thread per pixel (b, h, w) over its C channels.  In latent space y = decouple(x) (identity when inpainting,
+// y_j = sum_i x_i M_ij when colorizing), with a = mean coefficient and s = std of the data marginal at this step:
+//   y' = y*(1-m) + (a*known + s*z)*m,  x = couple(y'),  x_mean = couple(decouple(x)*(1-m) + (a*known)*m)
+// z is the blend's own torch.randn_like draw, regenerated per element (in the state's memory order: the reference's
+// colorization state is the channels-last output of its einsum, see PhiloxMap::nhwc).  Every product and sum is rounded separately
+// (no FMA contraction) in the reference's operation order, so the inpainting blend is bit-equal to the eager ops.
+__device__ __forceinline__ void mat3(const float* M, const float v[3], float y[3]) {   // y_j = sum_i v_i M[i*3+j]
+#pragma unroll
+  for (int j = 0; j < 3; ++j)
+    y[j] = __fadd_rn(__fadd_rn(__fmul_rn(v[0], M[j]), __fmul_rn(v[1], M[3 + j])), __fmul_rn(v[2], M[6 + j]));
+}
+
+__device__ __forceinline__ float blend(float y, float k, float m, float a, float s, float z) {
+  return __fadd_rn(__fmul_rn(y, __fsub_rn(1.f, m)), __fmul_rn(__fadd_rn(__fmul_rn(a, k), __fmul_rn(z, s)), m));
+}
+
+__device__ __forceinline__ float blend_mean(float y, float k, float m, float a) {
+  return __fadd_rn(__fmul_rn(y, __fsub_rn(1.f, m)), __fmul_rn(__fmul_rn(a, k), m));
+}
+
+__global__ void __launch_bounds__(256) pc_constrain_kernel(float* __restrict__ x, float* __restrict__ x_mean,
+                                                           const float* __restrict__ known, const float* __restrict__ mask,
+                                                           PhiloxMap m, const unsigned long long* offset_dev, const int* step,
+                                                           unsigned long long cps, unsigned long long cidx,
+                                                           const float* __restrict__ cm, const float* __restrict__ cs,
+                                                           PcColorTransform ct, int colorize, int C, long long HW) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  const int s_idx = step ? *step : 0;
+  const float a = cm[s_idx], s = cs[s_idx];
+  const unsigned long long off = step_offset(offset_dev, step, cps, cidx, m.inc);
+  const long long npix = m.numel / C;
+  for (long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x; p < npix; p += (long long)gridDim.x * blockDim.x) {
+    const long long b = p / HW, hw = p - b * HW;
+    const long long e0 = b * C * HW + hw;   // flat NCHW index of channel 0 at this pixel
+    if (colorize) {
+      float v[3], y[3], k[3], mk[3];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) { v[j] = x[e0 + j * HW]; k[j] = known[e0 + j * HW]; mk[j] = mask[e0 + j * HW]; }
+      mat3(ct.M, v, y);
+#pragma unroll
+      for (int j = 0; j < 3; ++j) y[j] = blend(y[j], k[j], mk[j], a, s, noise_at(m, off, draw_index(m, e0 + j * HW)));
+      mat3(ct.Minv, y, v);                     // x' = couple(y')
+#pragma unroll
+      for (int j = 0; j < 3; ++j) x[e0 + j * HW] = v[j];
+      mat3(ct.M, v, y);                        // decouple(x'), not y': the reference re-derives it from the blended x
+#pragma unroll
+      for (int j = 0; j < 3; ++j) y[j] = blend_mean(y[j], k[j], mk[j], a);
+      mat3(ct.Minv, y, v);
+#pragma unroll
+      for (int j = 0; j < 3; ++j) x_mean[e0 + j * HW] = v[j];
+    } else {
+      for (int c = 0; c < C; ++c) {
+        const long long e = e0 + c * HW;
+        const float k = known[e], mk = mask[e];
+        const float xn = blend(x[e], k, mk, a, s, noise_at(m, off, draw_index(m, e)));
+        x[e] = xn;
+        x_mean[e] = blend_mean(xn, k, mk, a);
+      }
     }
   }
 }
@@ -209,6 +288,23 @@ int launch_predictor_apply(float* x, float* x_mean, const float* out, const floa
   B200_REQUIRE(sc.pb != nullptr, "predictor_apply: pb table missing");
   launch_kernel(pc_apply_kernel, dim3(apply_grid(m)), dim3(256), 0, st, x, x_mean, out, noise, m, offset_dev, step, calls_per_step,
                                                  call_idx, nullptr, 0.f, sc, 1, add_noise);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+int launch_pc_constrain(float* x, float* x_mean, const float* known, const float* mask, const PhiloxMap& m,
+                        const unsigned long long* offset_dev, const int* step,
+                        unsigned long long calls_per_step, unsigned long long call_idx,
+                        const float* cm, const float* cs, const PcColorTransform& ct, int colorize, int C, long long HW,
+                        cudaStream_t st) {
+  B200_REQUIRE(x && x_mean && known && mask && cm && cs, "pc_constrain: null argument");
+  B200_REQUIRE(C > 0 && HW > 0 && m.numel % (C * HW) == 0, "pc_constrain: %lld elements are not whole %dx%lld images",
+               m.numel, C, HW);
+  B200_REQUIRE(!colorize || C == 3, "pc_constrain: colorization needs 3 channels, got %d", C);
+  const long long npix = m.numel / C;
+  const int grid = (int)std::min<long long>((npix + 255) / 256, 132LL * 16);
+  launch_kernel(pc_constrain_kernel, dim3(grid), dim3(256), 0, st, x, x_mean, known, mask, m, offset_dev, step,
+                calls_per_step, call_idx, cm, cs, ct, colorize, C, HW);
   B200_CHECK_LAUNCH();
   return 0;
 }

@@ -25,6 +25,11 @@ citing the reference statements it replaces:
 
 The per-step scalar tables are built here with the same torch fp32 ops the
 reference evaluates inside its loop, then handed to the C ABI as host arrays.
+
+``match_pc_plan(..., constraint='inpaint' | 'colorize')`` returns a
+:class:`ConstrainedPcPlan` for ``controllable_generation``: the same loop with
+the data-consistency blend (``controllable_generation.py:43-52`` / ``:137-146``)
+after the corrector block and after the predictor block of every iteration.
 """
 import ctypes
 
@@ -103,6 +108,17 @@ def build_tables(sde, predictor_kind, corrector_kind, probability_flow, eps, snr
   return out
 
 
+def build_constraint_tables(sde, eps):
+  """Per-step scalars of controllable generation's data-consistency blend (float32 numpy arrays of length N):
+  ``cm`` and ``cs`` with ``sde.marginal_prob(known, t_i) == (cm[i] * known, cs[i])`` (controllable_generation.py:44-45,
+  :138-139).  VE: ``cm = 1``, ``cs = sigma(t)``; (sub-)VP: ``cm = exp(log_mean_coeff(t))`` and the SDE's std."""
+  N = sde.N
+  t = torch.linspace(sde.T, eps, N)
+  cm, cs = sde.marginal_prob(torch.ones(N, 1, 1, 1), t)
+  f32 = lambda v: np.ascontiguousarray(v.reshape(N).to(torch.float32).numpy())
+  return dict(cm=f32(cm), cs=f32(cs))
+
+
 class PcPlan:
   """A native PC loop bound to one model, SDE, sampler configuration and batch shape."""
 
@@ -141,9 +157,10 @@ class PcPlan:
     cfg.n_corrector_steps = self.n_steps
     cfg.snr = self.snr
     fp = ctypes.POINTER(ctypes.c_float)
-    for k in ('label', 'score_scale', 'alpha', 'pa', 'pb', 'pc', 'ca', 'cb', 'cc'):
+    for k in ('label', 'score_scale', 'alpha', 'pa', 'pb', 'pc', 'ca', 'cb', 'cc', 'cm', 'cs'):
       if k in self.tables:
         setattr(cfg, k, self.tables[k].ctypes.data_as(fp))
+    self._configure(cfg)
     h = ctypes.c_void_p()
     _lib.call('b200_pc_create', eng['h'], ctypes.byref(cfg), self.shape[0], ctypes.byref(h))
     self._pc = h
@@ -153,8 +170,15 @@ class PcPlan:
       self._x = torch.empty(self.shape, dtype=torch.float32, device=self.device)
       self._xm = torch.empty(self.shape, dtype=torch.float32, device=self.device)
     _lib.call('b200_pc_bind_workspace', h, _lib.ptr(self._ws), self._ws.numel() * 4, _lib.stream_ptr(self.device))
+    self._bind(h)
     self._engine_id = key
     return eng
+
+  def _configure(self, cfg):
+    """Hook for variants: fill further ``PcConfig`` fields before the plan is created."""
+
+  def _bind(self, h):
+    """Hook for variants: bind further device buffers once the workspace is bound."""
 
   def _generator(self):
     idx = self.device.index if self.device.index is not None else torch.cuda.current_device()
@@ -195,6 +219,47 @@ class PcPlan:
     return int(_lib.load().b200_pc_launches_per_step(self._pc))
 
 
+class ConstrainedPcPlan(PcPlan):
+  """A :class:`PcPlan` for controllable generation: after the corrector block and after the predictor block of every
+  iteration the state is blended with a fresh draw from the data marginal (``constraint`` 'inpaint' or 'colorize',
+  controllable_generation.py:43-52 / :137-146).  ``known`` and ``mask`` live in persistent device buffers, so the
+  captured graph stays valid from one call to the next.  ``channels_last``: the state the reference loop draws its
+  ``randn_like`` noise on is channels-last, so torch fills it in NHWC memory order (the colorizer's einsum output)."""
+
+  def __init__(self, model, sde, predictor_kind, corrector_kind, shape, snr, n_steps, probability_flow, eps, device,
+               constraint, channels_last=False):
+    if constraint not in ('inpaint', 'colorize'):
+      raise ValueError(f'constraint must be inpaint or colorize, got {constraint!r}')
+    super().__init__(model, sde, predictor_kind, corrector_kind, shape, snr, n_steps, probability_flow, eps, device)
+    self.constraint, self.channels_last = constraint, bool(channels_last)
+    self.tables.update(build_constraint_tables(sde, eps))
+    self._known = self._mask = None
+
+  def _configure(self, cfg):
+    cfg.constraint = 1 if self.constraint == 'inpaint' else 2
+    cfg.noise_nhwc = int(self.channels_last)
+    if self.constraint == 'colorize':
+      from .controllable_generation import _M
+      m = torch.tensor(_M)
+      cfg.color_m[:] = m.flatten().tolist()
+      cfg.color_minv[:] = torch.inverse(m).flatten().tolist()   # the reference's invM, computed the same way
+
+  def _bind(self, h):
+    if self._known is None:
+      self._known = torch.empty(self.shape, dtype=torch.float32, device=self.device)
+      self._mask = torch.empty(self.shape, dtype=torch.float32, device=self.device)
+    _lib.call('b200_pc_bind_constraint', h, _lib.ptr(self._known), _lib.ptr(self._mask), _lib.stream_ptr(self.device))
+
+  def run(self, x, known, mask, first_step=0, num_steps=None, clone=True):
+    """:meth:`PcPlan.run` with the blend's ``known`` (the data; for colorization ``decouple(gray)``) and ``mask``
+    (1 where ``known`` is imposed).  A mask that broadcasts to the batch shape is expanded here."""
+    with torch.cuda.device(self.device):
+      self._ensure()
+      self._known.copy_(known.detach().expand(self.shape))
+      self._mask.copy_(mask.detach().expand(self.shape))
+      return super().run(x, first_step=first_step, num_steps=num_steps, clone=clone)
+
+
 def _kind_of_predictor(predictor):
   from . import sampling
   if predictor is None or predictor is sampling.NonePredictor:
@@ -219,8 +284,10 @@ def _kind_of_corrector(corrector):
   return None
 
 
-def match_pc_plan(sde, model, predictor, corrector, shape, snr, n_steps, probability_flow, continuous, eps, device):
-  """Return a :class:`PcPlan` when the native engine implements this sampler, else ``None``."""
+def match_pc_plan(sde, model, predictor, corrector, shape, snr, n_steps, probability_flow, continuous, eps, device,
+                  constraint=None, channels_last=False):
+  """Return a :class:`PcPlan` when the native engine implements this sampler, else ``None``.  With ``constraint``
+  'inpaint' or 'colorize' (controllable generation) the plan is a :class:`ConstrainedPcPlan`; the rules are the same."""
   from .models._engine import EngineModel
   model = _unwrap(model)
   if not isinstance(model, EngineModel) or torch.device(device).type != 'cuda' or not torch.cuda.is_available():
@@ -241,9 +308,15 @@ def match_pc_plan(sde, model, predictor, corrector, shape, snr, n_steps, probabi
       float(getattr(sde, a)) for a in ('sigma_min', 'sigma_max', 'beta_0', 'beta_1') if hasattr(sde, a))
   key = (sde_key, pk, ck, tuple(shape), float(snr), int(n_steps), bool(probability_flow), float(eps),
          str(model._explicit_device(device)))
+  if constraint is not None:
+    key += (constraint, bool(channels_last))
   cache = model.__dict__.setdefault('_pc_plans', {})
   plan = cache.get(key)
   if plan is None:
-    plan = PcPlan(model, sde, pk, ck, shape, snr, n_steps, probability_flow, eps, device)
+    if constraint is None:
+      plan = PcPlan(model, sde, pk, ck, shape, snr, n_steps, probability_flow, eps, device)
+    else:
+      plan = ConstrainedPcPlan(model, sde, pk, ck, shape, snr, n_steps, probability_flow, eps, device, constraint,
+                               channels_last)
     cache[key] = plan
   return plan
