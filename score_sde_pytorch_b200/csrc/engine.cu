@@ -151,15 +151,28 @@ int add_param(b200_ncsnpp* e, const std::string& name, std::vector<long long> sh
   return (int)e->params.size() - 1;
 }
 
+// Tensor-core convolution descriptor with the fields every contraction of the engine shares: A = a1 [C1] (+ a2 [C2])
+// over nimg images of H x W output pixels, W [taps][N][C1 + C2], one batch item, output pitch N, the engine's operand
+// format and halo mode.  The gemm sites switch conv off and set their own batch geometry.
+TcGemmDesc tc_desc(const b200_ncsnpp* e, const float* a1, int C1, const float* a2, int C2, int H, int W, int nimg, int taps,
+                   const float* w, int N) {
+  TcGemmDesc d; memset(&d, 0, sizeof(d));
+  d.f16 = e->cfg.precision == 2; d.no_halo = e->cfg.no_halo;
+  d.a1 = a1; d.C1 = C1; d.a2 = a2; d.C2 = C2; d.conv = 1; d.H = H; d.W = W; d.nimg = nimg; d.taps = taps;
+  d.w = w; d.N_total = N; d.K_total = C1 + C2; d.w_rows = (long long)taps * N; d.nbatch = 1; d.epi.ld_out = N;
+  return d;
+}
+
 // precision: 0 = tensor cores on TF32-grid fp32 operands, 1 = strict fp32 CUDA cores, 2 = tensor cores on fp16 operands
 // (same 11-bit significand as TF32, fp32 accumulation; half the operand bytes and twice the MMA rate)
 bool tc_ok(const b200_ncsnpp* e, int C1, int C2, int Cout, int H, int W, int taps) {
   if (e->cfg.precision == 1) return false;
-  TcGemmDesc d; memset(&d, 0, sizeof(d));
-  d.f16 = e->cfg.precision == 2;
-  d.C1 = C1; d.C2 = C2; d.a2 = C2 ? (const float*)1 : nullptr; d.conv = 1; d.H = H; d.W = W; d.nimg = 1; d.taps = taps;
-  d.N_total = Cout; d.K_total = C1 + C2; d.nbatch = 1; d.epi.ld_out = Cout; d.epi.ld_res = Cout;
-  return tc_gemm_supported(d, nullptr);
+  return tc_gemm_supported(tc_desc(e, nullptr, C1, C2 ? (const float*)1 : nullptr, C2, H, W, 1, taps, nullptr, Cout), nullptr);
+}
+
+bool has_attn(const b200_ncsnpp_config& c, int res) {
+  for (int i = 0; i < c.num_attn_resolutions; ++i) if (c.attn_resolutions[i] == res) return true;
+  return false;
 }
 
 int build_graph(b200_ncsnpp* e) {
@@ -192,7 +205,6 @@ int build_graph(b200_ncsnpp* e) {
   const int flatk = om == 2 ? 64 : 32;          // elements of one 128-byte K step (im2col contraction depth)
   std::vector<int> all_res(L);
   for (int i = 0; i < L; ++i) all_res[i] = c.image_size >> i;
-  auto has_attn = [&](int r) { for (int i = 0; i < c.num_attn_resolutions; ++i) if (c.attn_resolutions[i] == r) return true; return false; };
   // The positional embedding has no module in all_modules (ncsnpp.py:79-83): its Mod below takes no index, so every
   // later module's index is its position in `mods` minus one.
   const int ishift = c.embedding_type == 1 ? 1 : 0;
@@ -314,7 +326,7 @@ int build_graph(b200_ncsnpp* e) {
       const int out_ch = nf * c.ch_mult[lvl];
       add_resblock(in_ch, 0, out_ch, 0, 0, all_res[lvl]);
       in_ch = out_ch;
-      if (has_attn(all_res[lvl])) add_attn(in_ch, all_res[lvl]);
+      if (has_attn(c, all_res[lvl])) add_attn(in_ch, all_res[lvl]);
       hs_c.push_back(in_ch);
     }
     if (lvl != L - 1) {
@@ -353,7 +365,7 @@ int build_graph(b200_ncsnpp* e) {
       add_resblock(in_ch, skip, out_ch, 0, 0, all_res[lvl]);
       in_ch = out_ch;
     }
-    if (has_attn(all_res[lvl])) add_attn(in_ch, all_res[lvl]);
+    if (has_attn(c, all_res[lvl])) add_attn(in_ch, all_res[lvl]);
     if (c.progressive == 1) {
       // output_skip (ncsnpp.py:190-203, 325-341): GroupNorm + SiLU + conv3x3 (in_ch -> image channels) at every level;
       // the image-channel pyramid is upsampled and summed, and IS the network output
@@ -398,6 +410,26 @@ int build_graph(b200_ncsnpp* e) {
 // ---------------------------------------------------------------------------
 // Plan builder
 // ---------------------------------------------------------------------------
+// GroupNorm coefficient tables for the few-channel convolutions that normalise while staging their input
+struct Coef { float* scale = nullptr; float* shift = nullptr; long long bytes = 0; };
+
+// optional arguments of conv(), set by name: conv(..., Conv().taps(1).residual(x).scale(s).stats())
+struct Conv {
+  int taps_ = 9, stride_ = 1, Hin_ = 0, round_ = 0, row_ = -1, skip_w_ = -1, skip_b_ = -1;
+  Tensor residual_, skip1_, skip2_;
+  float scale_ = 1.f; bool stats_ = false; const Coef* gn_ = nullptr;
+  Conv& taps(int t) { taps_ = t; return *this; }                        // 9 (3x3) or 1 (1x1)
+  Conv& stride(int s, int Hin) { stride_ = s; Hin_ = Hin; return *this; }   // stride 2: VALID over Hin x Hin inputs
+  Conv& residual(const Tensor& r) { residual_ = r; return *this; }      // out = (acc + bias + residual) * scale
+  Conv& scale(float s) { scale_ = s; return *this; }
+  Conv& round(int r) { round_ = r; return *this; }                      // output format (store_operand4 mode)
+  Conv& stats() { stats_ = true; return *this; }                        // GroupNorm quad sums of the output, when fused
+  Conv& temb(int dense_row) { row_ = dense_row; return *this; }         // + this block's Dense_0 row of the time embedding
+  // fused skip projection: the 1x1 conv (weights pw, bias pb) of x1 (+ x2) as extra K steps (tensor-core path)
+  Conv& skip(const Tensor& x1, const Tensor& x2, int pw, int pb) { skip1_ = x1; skip2_ = x2; skip_w_ = pw; skip_b_ = pb; return *this; }
+  Conv& gn(const Coef& c) { gn_ = &c; return *this; }                   // GroupNorm+SiLU on load (few-channel kernel)
+};
+
 struct Builder {
   b200_ncsnpp* e; int B; char* base; bool dry; Arena arena; int rc = 0;
   char* stats_base = nullptr; long long stats_top = 0;   // bump region for GroupNorm quad sums, zeroed once per forward
@@ -408,7 +440,11 @@ struct Builder {
   std::string next_name;                       // label of the next op (shape summary for the per-op profile)
   double next_bytes = 0.0;                     // algorithmic HBM bytes of the next op
   bool tan = false;                            // tangent plan (cfg.tangent): every tensor carries its tangent in Tensor::d
-  bool tan_op = false;                         // the op being added is a tangent op (labelled "tangent[...]")
+  bool tan_op = false;                         // the op being added is a tangent op (labelled "tangent[...]"); set by tangent()
+  size_t mi = 3;                               // next module of e->mods to plan (0..2: the time embedding)
+  const float* dense_all_ = nullptr;           // Dense_0 rows of every resblock [B][sumC]
+  Tensor pyr; bool pyr_nchw = true, pyr_owned = false; long long pyr_bytes = 0;   // input pyramid (progressive_input)
+  float* opyr = nullptr; long long opyr_bytes = 0;      // output_skip pyramid [B][ch][H][W] of the previous (coarser) level
   void name(const char* fmt, ...) {
     char buf[160]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap); next_name = buf;
   }
@@ -461,6 +497,29 @@ struct Builder {
     next_name.clear(); next_bytes = 0.0;
   }
 
+  // A linear op and, in tangent plans, its tangent twin: emit(false) adds the op on the primal buffers, emit(true) the same
+  // op on the tangent buffers (Tensor::d, no bias, J v into tout), which op() labels "tangent[separate]: " + the label.
+  template <class F> void twin(F emit) {
+    emit(false);
+    if (tan) tangent([&] { emit(true); });
+  }
+  // ops of tangent plans that are not copies of a primal op: gn_tangent, softmax_tangent, the attention product rule
+  template <class F> void tangent(F emit) { tan_op = true; emit(); tan_op = false; }
+
+  const Mod& next() { return e->mods[mi++]; }
+  // the block output nh replaces the running activation h (freed) and is recorded as module m's output
+  void advance(Tensor& h, const Mod& m, const Tensor& nh) { tfree(h); h = nh; tap(m.index, h); }
+
+  // CUDA-core / few-channel convolution descriptor over the B images of this plan: x1 [B][H][W][C1] -> [B][OH][OW][N] with
+  // `taps` (9: 3x3, 'same' padding at stride 1, VALID at stride 2; 1: 1x1), weights w [taps][N][C1]; unit epilogue
+  SimtConv simt_desc(const float* x1, int C1, int H, int W, int taps, int stride, int OH, int OW, const float* w, int N) const {
+    SimtConv s; memset(&s, 0, sizeof(s));
+    s.x1 = x1; s.C1 = C1; s.in_scale = 1.f; s.H = H; s.W = W; s.R = s.S = (taps == 9 ? 3 : 1); s.stride = stride;
+    s.pad = (taps == 9 && stride == 1 ? 1 : 0); s.OH = OH; s.OW = OW; s.nbatch = B; s.a_batched = 1; s.w = w; s.N = N;
+    s.epi.scale = 1.f; s.epi.rows_per_img = OH * OW; s.epi.ld_out = N; s.epi.ld_res = N;
+    return s;
+  }
+
   // make sure tensor t has quad sums: produced by its tensor-core epilogue, else by one streaming pass
   void ensure_qs(Tensor& t) {
     if (t.qs || !t.p) return;
@@ -499,15 +558,13 @@ struct Builder {
                   const float* mr, int G, int HW) {
     const int Bc = B;
     name("gn_tangent %d+%d @%d%s%s (%s stats)", a.C, b.C, a.H, act ? " silu" : "", draw ? " +raw" : "", mr ? "generic" : "quad");
-    tan_op = true;
-    op(1, [=](cudaStream_t st) {
-      return launch_gn_tangent(a.p, a.d, a.C, b.p, b.d, b.C, a.qs, b.qs, mr, g, bt, Bc, HW, G, 1e-6f, act, round, y.d, draw, st);
-    }, 2);
-    tan_op = false;
+    tangent([&] {
+      op(1, [=](cudaStream_t st) {
+        return launch_gn_tangent(a.p, a.d, a.C, b.p, b.d, b.C, a.qs, b.qs, mr, g, bt, Bc, HW, G, 1e-6f, act, round, y.d, draw, st);
+      }, 2);
+    });
   }
 
-  // ---- GroupNorm coefficient tables for the few-channel convolutions that normalise while staging their input ----
-  struct Coef { float* scale = nullptr; float* shift = nullptr; long long bytes = 0; };
   Coef gncoef(Tensor& x1, Tensor& x2, int pgw, int pgb) {
     const int C = x1.C + x2.C, G = groups(C), HW = x1.H * x1.W;
     ensure_qs(x1); ensure_qs(x2);
@@ -554,34 +611,42 @@ struct Builder {
     }, 3);
   }
 
-  // 3x3 / 1x1 'same' convolution on NHWC tensors, stride 1.
-  void conv(bool use_tc, Tensor a1, Tensor a2, int taps, int pw, int pb, int Cout, int dense_row /* -1 = none */,
-            const float* residual, float scale, int round, Tensor& out, bool want_stats = false, int stride = 1,
-            int Hin = 0, Tensor x3 = Tensor(), Tensor x4 = Tensor(), int pw2 = -1, int pb2 = -1, const Coef* gnc = nullptr) {
+  // 3x3 / 1x1 convolution on NHWC tensors into out (out.C channels), stride 1 'same' or stride 2 VALID.  In tangent plans
+  // it is followed by its tangent: the same contraction over the tangents of the operands and of the residual, without
+  // bias, time-embedding row or GroupNorm sums.
+  void conv(bool use_tc, const Tensor& a1, const Tensor& a2, int pw, int pb, Tensor& out, const Conv& o = Conv()) {
+    twin([&](bool d) {
+      if (!d) return conv_op(use_tc, a1, a2, pw, pb, out, o);
+      Conv t = o; t.residual_ = tg(o.residual_); t.row_ = -1; t.stats_ = false;
+      Tensor dout = tg(out);
+      conv_op(use_tc, tg(a1), tg(a2), pw, -1, dout, t);
+    });
+  }
+  void conv_op(bool use_tc, const Tensor& a1, const Tensor& a2, int pw, int pb, Tensor& out, const Conv& o) {
+    const int Cout = out.C, taps = o.taps_, stride = o.stride_, Hin = o.Hin_, dense_row = o.row_;
+    const Tensor &x3 = o.skip1_, &x4 = o.skip2_;
+    const float* residual = o.residual_.p;
     Epilogue ep; memset(&ep, 0, sizeof(ep));
     ep.bias = pb >= 0 ? e->W(pb) : nullptr;   // pb < 0: no bias (tangent ops)
     ep.rowvec = nullptr;   // patched at launch (depends on the per-call buffers)
-    ep.residual = residual; ep.ld_res = Cout; ep.scale = scale; ep.round_tf32 = round;
+    ep.residual = residual; ep.ld_res = Cout; ep.scale = o.scale_; ep.round_tf32 = o.round_;
     ep.rows_per_img = out.H * out.W; ep.out = out.p; ep.ld_out = Cout;
     b200_ncsnpp* eng = e;
     const float* dense_all = dense_all_;
     const int sumC = e->sumC;
     const double cflops = 2.0 * B * out.H * out.W * (double)Cout * ((a1.C + a2.C) * taps + x3.C + x4.C);
     if (x3.p && !use_tc) { set_error("ncsnpp: fused skip projection needs the tensor-core path"); rc = 2; return; }
-    if (gnc && use_tc) { set_error("ncsnpp: conv(): GroupNorm coefficients go with the few-channel kernel (the tensor-core path reads normalised operands)"); rc = 2; return; }
+    if (o.gn_ && use_tc) { set_error("ncsnpp: conv(): GroupNorm coefficients go with the few-channel kernel (the tensor-core path reads normalised operands)"); rc = 2; return; }
     if (use_tc) {
-      TcGemmDesc d; memset(&d, 0, sizeof(d));
-      d.a1 = a1.p; d.C1 = a1.C; d.a2 = a2.p; d.C2 = a2.C; d.conv = 1; d.H = out.H; d.W = out.W; d.nimg = B; d.taps = taps;
+      TcGemmDesc d = tc_desc(e, a1.p, a1.C, a2.p, a2.C, out.H, out.W, B, taps, e->W(pw), Cout);
       d.stride = stride; d.valid_pad = stride == 2 ? 1 : 0; d.Hin = Hin ? Hin : out.H; d.Win = Hin ? Hin : out.W;
-      d.w = e->W(pw); d.N_total = Cout; d.K_total = a1.C + a2.C; d.w_rows = (long long)taps * Cout; d.nbatch = 1;
-      d.f16 = om == 2; d.no_halo = e->cfg.no_halo;
       if (dense_row >= 0) ep.rowvec = dense_all + dense_row;
       if (x3.p) {   // fused skip projection: its bias rides in the (image-independent) row-vector slot
         if (dense_row >= 0) { set_error("ncsnpp: fused skip projection on a conv with a time-embedding bias"); rc = 2; return; }
-        d.a3 = x3.p; d.C3 = x3.C; d.a4 = x4.p; d.C4 = x4.C; d.w2 = e->W(pw2);
-        ep.rowvec = e->W(pb2); ep.rowvec_ld = 0;
+        d.a3 = x3.p; d.C3 = x3.C; d.a4 = x4.p; d.C4 = x4.C; d.w2 = e->W(o.skip_w_);
+        ep.rowvec = e->W(o.skip_b_); ep.rowvec_ld = 0;
       }
-      if (want_stats && fused_stats && (ep.rows_per_img % 32 == 0 || ep.rows_per_img == 16)) { out.qs = qalloc(Cout); d.qstats = out.qs; }
+      if (o.stats_ && fused_stats && (ep.rows_per_img % 32 == 0 || ep.rows_per_img == 16)) { out.qs = qalloc(Cout); d.qstats = out.qs; }
       d.epi = ep;
       if (dry) return;
       TcGemmPlan* pl = nullptr;
@@ -593,7 +658,7 @@ struct Builder {
       {
         const double es = om == 2 ? 2.0 : 4.0, px = (double)B * out.H * out.W;
         const double in_px = (double)B * (Hin ? (double)Hin * Hin : (double)out.H * out.W);
-        next_bytes = in_px * (a1.C + a2.C) * es + px * (x3.C + x4.C) * es + px * Cout * (round == 2 ? 2.0 : 4.0) +
+        next_bytes = in_px * (a1.C + a2.C) * es + px * (x3.C + x4.C) * es + px * Cout * (o.round_ == 2 ? 2.0 : 4.0) +
                      (residual ? px * Cout * 4.0 : 0.0) + ((double)taps * (a1.C + a2.C) + x3.C + x4.C) * Cout * es;
       }
       op(1, [=](cudaStream_t st) {
@@ -601,22 +666,20 @@ struct Builder {
         return tc_gemm_launch(pl, st);
       }, 0, cflops);
     } else {
-      SimtConv s; memset(&s, 0, sizeof(s));
-      s.x1 = a1.p; s.C1 = a1.C; s.x2 = a2.p; s.C2 = a2.C; s.in_scale = 1.f; s.in_shift = 0.f;
-      s.H = a1.H; s.W = a1.W; s.R = s.S = (taps == 9 ? 3 : 1); s.stride = 1; s.pad = (taps == 9 ? 1 : 0);
-      s.OH = a1.H; s.OW = a1.W; s.nbatch = B; s.a_batched = 1; s.w = e->W(pw); s.N = Cout;
+      SimtConv s = simt_desc(a1.p, a1.C, a1.H, a1.W, taps, 1, a1.H, a1.W, e->W(pw), Cout);
+      s.x2 = a2.p; s.C2 = a2.C;
       if (dense_row >= 0) ep.rowvec = dense_all + dense_row;
       s.epi = ep;
       // few-channel levels of the nf = 16 networks: warp-level TF32 MMAs keep them at the HBM roofline (conv_lowc.cu);
       // strict-fp32 mode and every other shape stay on the CUDA-core kernel
       // (tangent plans keep every level on the CUDA-core kernel)
       const bool lowc = e->cfg.precision != 1 && !tan && !a1.f16 && !a2.f16 && sumC % 2 == 0 && conv_lowc_supported(s);
-      if (want_stats && lowc && fused_stats) { out.qs = qalloc(Cout); s.qstats = out.qs; }   // the epilogue sums what the next GroupNorm needs
-      if (gnc) {
+      if (o.stats_ && lowc && fused_stats) { out.qs = qalloc(Cout); s.qstats = out.qs; }   // the epilogue sums what the next GroupNorm needs
+      if (o.gn_) {
         if (!lowc) { set_error("ncsnpp: GroupNorm on load planned for a convolution the few-channel kernel does not take"); rc = 2; return; }
-        s.gn_scale = gnc->scale; s.gn_shift = gnc->shift; s.gn_act = 1;
+        s.gn_scale = o.gn_->scale; s.gn_shift = o.gn_->shift; s.gn_act = 1;
       }
-      name("conv%s %s%d+%d->%d @%d [%s]", taps == 9 ? "3x3" : "1x1", gnc ? "gn+silu " : "", a1.C, a2.C, Cout, out.H, lowc ? "mma.sync tf32" : "cuda-core");
+      name("conv%s %s%d+%d->%d @%d [%s]", taps == 9 ? "3x3" : "1x1", o.gn_ ? "gn+silu " : "", a1.C, a2.C, Cout, out.H, lowc ? "mma.sync tf32" : "cuda-core");
       next_bytes = (double)B * out.H * out.W * ((a1.C + a2.C) * 4.0 + Cout * 4.0 + (residual ? Cout * 4.0 : 0.0)) +
                    (double)taps * (a1.C + a2.C) * Cout * 4.0;
       op(1, [=](cudaStream_t st) {
@@ -625,17 +688,6 @@ struct Builder {
         return lowc ? launch_conv_lowc(c, st) : launch_conv_simt(c, st);
       }, lowc ? 7 : 1, cflops);
     }
-  }
-
-  // tangent of conv(): the same contraction over the tangents of its operands, without bias and time-embedding row;
-  // dres: the tangent of the residual
-  void conv_t(bool use_tc, const Tensor& a1, const Tensor& a2, int taps, int pw, int Cout, const float* dres, float scale, int round,
-              const Tensor& out, int stride = 1, int Hin = 0) {
-    if (!tan) return;
-    Tensor o = tg(out);
-    tan_op = true;
-    conv(use_tc, tg(a1), tg(a2), taps, pw, -1, Cout, -1, dres, scale, round, o, /*want_stats=*/false, stride, Hin);
-    tan_op = false;
   }
 
   // batched C[b] = A[b] * W[b]^T
@@ -647,11 +699,9 @@ struct Builder {
     ep.bias = bias; ep.residual = residual; ep.ld_res = ld_res; ep.scale = scale; ep.round_tf32 = round;
     ep.rows_per_img = rows_per_img; ep.out = out; ep.ld_out = ldo;
     if (use_tc) {
-      TcGemmDesc d; memset(&d, 0, sizeof(d));
-      d.a1 = A; d.C1 = K; d.conv = 0; d.taps = 1; d.a_rows = a_rows; d.a_ld = lda; d.a_batch_rows = a_batch_rows;
-      d.w = Wm; d.N_total = N; d.K_total = K; d.w_rows = w_rows; d.w_ld = ldw; d.w_batch_rows = w_batch_rows;
-      d.nbatch = nbatch; d.M_per_batch = M; d.qstats = qstats; d.epi = ep;
-      d.f16 = om == 2;
+      TcGemmDesc d = tc_desc(e, A, K, nullptr, 0, 0, 0, 0, 1, Wm, N);
+      d.conv = 0; d.a_rows = a_rows; d.a_ld = lda; d.a_batch_rows = a_batch_rows;
+      d.w_rows = w_rows; d.w_ld = ldw; d.w_batch_rows = w_batch_rows; d.nbatch = nbatch; d.M_per_batch = M; d.qstats = qstats; d.epi = ep;
       if (dry) return;
       TcGemmPlan* pl = nullptr;
       if (int r = tc_gemm_plan_create(d, &pl)) { rc = r; return; }
@@ -664,24 +714,21 @@ struct Builder {
       }
       op(1, [=](cudaStream_t st) { return tc_gemm_launch(pl, st); }, 0, 2.0 * nbatch * (double)M * N * K);
     } else {
-      SimtConv s; memset(&s, 0, sizeof(s));
-      s.x1 = A; s.C1 = K; s.ld1 = lda; s.in_scale = 1.f; s.H = M; s.W = 1; s.R = s.S = 1; s.stride = 1; s.pad = 0;
-      s.OH = M; s.OW = 1; s.nbatch = nbatch; s.a_batched = a_batch_rows != 0; s.w = Wm; s.N = N;
+      SimtConv s = simt_desc(A, K, M, 1, 1, 1, M, 1, Wm, N);
+      s.ld1 = lda; s.nbatch = nbatch; s.a_batched = a_batch_rows != 0;
       s.w_batch_stride = (long long)w_batch_rows * ldw; s.w_ld = ldw;
       ep.rows_per_img = M; s.epi = ep;
       op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * nbatch * (double)M * N * K);
     }
   }
 
-  const float* dense_all_ = nullptr;
   void tap(int idx, const Tensor& t) { if (!dry) e->taps[idx] = t; }
 
   // would conv() run this stride-1 convolution on the few-channel kernel (conv_lowc.cu: TF32 mode, fp32 tensors)?
   bool lowc_ok(int C1, int C2, int Cout, int H, int taps) const {
     if (e->cfg.precision != 0 || e->sumC % 2 != 0) return false;
-    SimtConv s; memset(&s, 0, sizeof(s));
-    s.C1 = C1; s.C2 = C2; s.in_scale = 1.f; s.H = H; s.W = H; s.R = s.S = (taps == 9 ? 3 : 1); s.stride = 1; s.pad = (taps == 9 ? 1 : 0);
-    s.OH = H; s.OW = H; s.nbatch = B; s.a_batched = 1; s.N = Cout; s.epi.ld_out = Cout; s.epi.ld_res = Cout;
+    SimtConv s = simt_desc(nullptr, C1, H, H, taps, 1, H, H, nullptr, Cout);
+    s.C2 = C2;
     return conv_lowc_supported(s);
   }
 
@@ -709,14 +756,10 @@ struct Builder {
       Tensor a0r = talloc(Cin, Ho, Ho);
       xr = talloc(Cin, Ho, Ho);
       xr.f16 = m.tc2 && om == 2;
-      resample2x(a0.p, H, Cin, m.up != 0, m.tc0 ? om : 0, a0r.p);
-      resample2x(x1.p, H, Cin, m.up != 0, m.tc2 ? om : 0, xr.p);
-      if (tan) {   // the resampling is linear: the same kernels on the tangents
-        tan_op = true;
-        resample2x(a0.d, H, Cin, m.up != 0, m.tc0 ? om : 0, a0r.d);
-        resample2x(x1.d, H, Cin, m.up != 0, m.tc2 ? om : 0, xr.d);
-        tan_op = false;
-      }
+      twin([&](bool d) {
+        resample2x(d ? a0.d : a0.p, H, Cin, m.up != 0, m.tc0 ? om : 0, d ? a0r.d : a0r.p);
+        resample2x(d ? x1.d : x1.p, H, Cin, m.up != 0, m.tc2 ? om : 0, d ? xr.d : xr.p);
+      });
       tfree(a0); a0 = a0r;
     }
     Tensor h1 = talloc(m.cout, Ho, Ho);
@@ -725,11 +768,10 @@ struct Builder {
     h1.f16 = h1_f16;
     if (lc0) {
       Coef c0 = gncoef(x1, x2, m.gn0w, m.gn0b);
-      conv(false, x1, x2, 9, m.c0w, m.c0b, m.cout, m.dense_row, nullptr, 1.f, 0, h1, /*want_stats=*/true, 1, 0, Tensor(), Tensor(), -1, -1, &c0);
+      conv(false, x1, x2, m.c0w, m.c0b, h1, Conv().temb(m.dense_row).stats().gn(c0));
       ffree(c0.scale, c0.bytes);
     } else {
-      conv(m.tc0, a0, Tensor(), 9, m.c0w, m.c0b, m.cout, m.dense_row, nullptr, 1.f, h1_f16 ? 2 : 0, h1, /*want_stats=*/true);
-      conv_t(m.tc0, a0, Tensor(), 9, m.c0w, m.cout, nullptr, 1.f, 0, h1);
+      conv(m.tc0, a0, none, m.c0w, m.c0b, h1, Conv().temb(m.dense_row).round(h1_f16 ? 2 : 0).stats());
       tfree(a0);
     }
     if (h1_f16 && !h1.qs) { set_error("ncsnpp: fp16 mid-block tensor without fused GroupNorm sums"); rc = 2; return Tensor(); }
@@ -742,39 +784,32 @@ struct Builder {
       tfree(h1);
     }
     Tensor s;
-    const float* residual = x1.p;
-    const float* dresidual = x1.d;
+    Tensor residual = x1;
     // Fused skip projection (default): Conv_2(x) (layerspp.py:270) is accumulated inside the second 3x3 convolution
     // as extra K steps instead of a separate launch + a residual round trip through HBM.  (Tangent plans: its bias rides
     // in the row-vector slot, so the skip projection stays a contraction of its own there.)
     if (m.has_conv2 && m.tc1 && m.tc2 && (resample || raw.p) && !tan) {
       Tensor out = talloc(m.cout, Ho, Ho);
-      Tensor e1 = resample ? xr : raw, e2 = Tensor();
+      Tensor e1 = resample ? xr : raw;
       e1.f16 = false;   // conv() addresses operands by the engine-wide operand mode
-      conv(true, a1, Tensor(), 9, m.c1w, m.c1b, m.cout, -1, nullptr, inv_s2, 0, out, /*want_stats=*/true, 1, 0, e1, e2, m.c2w, m.c2b);
+      conv(true, a1, none, m.c1w, m.c1b, out, Conv().scale(inv_s2).stats().skip(e1, none, m.c2w, m.c2b));
       tfree(a1); tfree(raw); tfree(xr);
       return out;
     }
     if (m.has_conv2) {
       s = talloc(m.cout, Ho, Ho);
-      if (resample) { conv(m.tc2, xr, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-                      conv_t(m.tc2, xr, Tensor(), 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
-      else if (m.tc2 && raw.p) { conv(true, raw, Tensor(), 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-                                 conv_t(true, raw, Tensor(), 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
-      else if (m.tc2) { conv(true, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-                        conv_t(true, x1, x2, 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
-      else { conv(false, x1, x2, 1, m.c2w, m.c2b, m.cout, -1, nullptr, 1.f, 0, s);
-             conv_t(false, x1, x2, 1, m.c2w, m.cout, nullptr, 1.f, 0, s); }
-      residual = s.p; dresidual = s.d;
+      if (resample) conv(m.tc2, xr, none, m.c2w, m.c2b, s, Conv().taps(1));
+      else if (m.tc2 && raw.p) conv(true, raw, none, m.c2w, m.c2b, s, Conv().taps(1));
+      else conv(m.tc2, x1, x2, m.c2w, m.c2b, s, Conv().taps(1));
+      residual = s;
       tfree(raw); tfree(xr);
     } else if (x2.p) { set_error("ncsnpp: concat input without a skip convolution"); rc = 2; return Tensor(); }
     Tensor out = talloc(m.cout, Ho, Ho);
     if (lc1) {
-      conv(false, h1, Tensor(), 9, m.c1w, m.c1b, m.cout, -1, residual, inv_s2, 0, out, /*want_stats=*/true, 1, 0, Tensor(), Tensor(), -1, -1, &c1);
+      conv(false, h1, none, m.c1w, m.c1b, out, Conv().residual(residual).scale(inv_s2).stats().gn(c1));
       ffree(c1.scale, c1.bytes); tfree(h1);
     } else {
-      conv(m.tc1, a1, Tensor(), 9, m.c1w, m.c1b, m.cout, -1, residual, inv_s2, 0, out, /*want_stats=*/true);
-      conv_t(m.tc1, a1, Tensor(), 9, m.c1w, m.cout, dresidual, inv_s2, 0, out);
+      conv(m.tc1, a1, none, m.c1w, m.c1b, out, Conv().residual(residual).scale(inv_s2).stats());
       tfree(a1);
     }
     tfree(s);
@@ -815,16 +850,13 @@ struct Builder {
       float *dqk = nullptr, *dvT = nullptr, *dS = nullptr;   // tangents (tangent plans)
       float* qk = falloc2((long long)B * T * 2 * C, &qkb, &dqk);
       float* vT = falloc2((long long)B * C * T, &vtb, &dvT);
-      // q,k = a Wq^T + bq | a Wk^T + bk   (layerspp.py:78-79) in one N=2C contraction
-      gemm(tc, a.p, C, BT, 0 /* rows enumerated flat */, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, bqkv, nullptr, 0, 1.f, tc ? om : 0, qk, 2 * C);
-      // v^T[b][c][t] = sum_i Wv[c][i] a[b][t][i]   (bias bv is added after the PV product: softmax rows sum to 1)
-      gemm(tc, wv, C, C, 0, a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, vT, T, nullptr, 1 << 30);
-      if (tan) {   // dq, dk, dv: the projections of da, without bias
-        tan_op = true;
-        gemm(tc, a.d, C, BT, 0, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, dqk, 2 * C);
-        gemm(tc, wv, C, C, 0, a.d, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, dvT, T, nullptr, 1 << 30);
-        tan_op = false;
-      }
+      twin([&](bool d) {   // tangent: dq, dk, dv, the projections of da without bias
+        // q,k = a Wq^T + bq | a Wk^T + bk   (layerspp.py:78-79) in one N=2C contraction
+        gemm(tc, d ? a.d : a.p, C, BT, 0 /* rows enumerated flat */, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, d ? nullptr : bqkv,
+             nullptr, 0, 1.f, tc ? om : 0, d ? dqk : qk, 2 * C);
+        // v^T[b][c][t] = sum_i Wv[c][i] a[b][t][i]   (bias bv is added after the PV product: softmax rows sum to 1)
+        gemm(tc, wv, C, C, 0, d ? a.d : a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, d ? dvT : vT, T, nullptr, 1 << 30);
+      });
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
       // [T,T] logits/probabilities and the attention output stay on chip; other token counts (tf32 mode) use separate launches.
@@ -853,10 +885,10 @@ struct Builder {
       gemm(tc, qk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30);
       if (tan) {   // dS = dq k^T + q dk^T
         long long tb; float* t1 = falloc(BT * T, &tb);
-        tan_op = true;
-        gemm(tc, dqk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, t1, T, nullptr, 1 << 30);
-        gemm(tc, qk, 2 * C, BT, T, dqk + C, 2 * C, BT, T, B, T, T, C, nullptr, t1, T, 1.f, 0, dS, T, nullptr, 1 << 30);
-        tan_op = false;
+        tangent([&] {
+          gemm(tc, dqk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, t1, T, nullptr, 1 << 30);
+          gemm(tc, qk, 2 * C, BT, T, dqk + C, 2 * C, BT, T, B, T, T, C, nullptr, t1, T, 1.f, 0, dS, T, nullptr, 1 << 30);
+        });
         ffree(t1, tb);
       }
       ffree(qk, qkb);
@@ -864,27 +896,24 @@ struct Builder {
       op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
       if (tan) {   // dP = P (sc dS - rowsum(P sc dS)), over dS
         name("softmax_tangent T=%d", T);
-        tan_op = true;
-        op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
-        tan_op = false;
+        tangent([&] { op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4); });
       }
       O = falloc2(BT * C, &ob, &dO);
       // h[b][q][c] = sum_k P[q][k] v[k][c] + bv[c]   (layerspp.py:86)
       gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? 1 : 0, O, C);
       if (tan) {   // dO = dP v + P dv
         long long tb; float* t2 = falloc(BT * C, &tb);
-        tan_op = true;
-        gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
-        gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? 1 : 0, dO, C);
-        tan_op = false;
+        tangent([&] {
+          gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
+          gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? 1 : 0, dO, C);
+        });
         ffree(t2, tb);
       }
       ffree(S, sb); ffree(vT, vtb);
     }
     Tensor out = talloc(C, x.H, x.W);
     Tensor Ot; Ot.p = O; Ot.C = C; Ot.H = x.H; Ot.W = x.W; Ot.d = dO;
-    conv(m.tc2, Ot, Tensor(), 1, m.nw[3], m.nb[3], C, -1, x.p, inv_s2, 0, out, /*want_stats=*/true);   // NIN_3 + (x+h)/sqrt2 (:87-91)
-    conv_t(m.tc2, Ot, Tensor(), 1, m.nw[3], C, x.d, inv_s2, 0, out);
+    conv(m.tc2, Ot, none, m.nw[3], m.nb[3], out, Conv().taps(1).residual(x).scale(inv_s2).stats());   // NIN_3 + (x+h)/sqrt2 (:87-91)
     ffree(O, ob);
     return out;
   }
@@ -898,34 +927,22 @@ struct Builder {
     if (m.tc0) {
       // the block output is fp32; the tensor cores read it in the operand format (TF32 grid / fp16)
       Tensor xo = talloc(x.C, H, H);
-      const float* src = x.p; float* dst = xo.p; const long long n = (long long)B * H * H * x.C; const int omc = om;
-      name("operand copy %d @%d", x.C, H);
-      next_bytes = (double)n * (4.0 + (om == 2 ? 2.0 : 4.0));
-      op(1, [=](cudaStream_t st) { return launch_store_operand(src, dst, n, omc, st); }, 6);
-      if (tan) {
-        const float* dsrc = x.d; float* ddst = xo.d;
+      const long long n = (long long)B * H * H * x.C; const int omc = om;
+      twin([&](bool d) {
+        const float* src = d ? x.d : x.p; float* dst = d ? xo.d : xo.p;
         name("operand copy %d @%d", x.C, H);
-        tan_op = true;
-        op(1, [=](cudaStream_t st) { return launch_store_operand(dsrc, ddst, n, omc, st); }, 6);
-        tan_op = false;
-      }
-      conv(true, xo, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true, /*stride=*/2, /*Hin=*/H);
-      conv_t(true, xo, Tensor(), 9, m.w, m.cout, nullptr, 1.f, 0, out, /*stride=*/2, /*Hin=*/H);
+        next_bytes = (double)n * (4.0 + (om == 2 ? 2.0 : 4.0));
+        op(1, [=](cudaStream_t st) { return launch_store_operand(src, dst, n, omc, st); }, 6);
+      });
+      conv(true, xo, Tensor(), m.w, m.b, out, Conv().stats().stride(2, H));
       tfree(xo);
     } else {
-      SimtConv s; memset(&s, 0, sizeof(s));
-      s.x1 = x.p; s.C1 = x.C; s.in_scale = 1.f; s.H = H; s.W = H; s.R = s.S = 3; s.stride = 2; s.pad = 0;
-      s.OH = Ho; s.OW = Ho; s.nbatch = B; s.a_batched = 1; s.w = e->W(m.w); s.N = m.cout;
-      s.epi.bias = e->W(m.b); s.epi.scale = 1.f; s.epi.rows_per_img = Ho * Ho; s.epi.out = out.p; s.epi.ld_out = m.cout;
-      name("conv3x3 s2 %d->%d @%d [cuda-core]", x.C, m.cout, Ho);
-      op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
-      if (tan) {
-        SimtConv sd = s; sd.x1 = x.d; sd.epi.bias = nullptr; sd.epi.out = out.d;
+      twin([&](bool d) {
+        SimtConv s = simt_desc(d ? x.d : x.p, x.C, H, H, 9, 2, Ho, Ho, e->W(m.w), m.cout);
+        s.epi.bias = d ? nullptr : e->W(m.b); s.epi.out = d ? out.d : out.p;
         name("conv3x3 s2 %d->%d @%d [cuda-core]", x.C, m.cout, Ho);
-        tan_op = true;
-        op(1, [=](cudaStream_t st) { return launch_conv_simt(sd, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
-        tan_op = false;
-      }
+        op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * Ho * Ho * (double)m.cout * x.C * 9);
+      });
     }
     return out;
   }
@@ -935,322 +952,291 @@ struct Builder {
   Tensor upsample(const Mod& m, Tensor& x) {
     const int H = x.H, Ho = 2 * H;
     Tensor u = talloc(x.C, Ho, Ho);
-    fir(x.p, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, u.p, 1.f, /*box=*/true);
-    if (tan) { tan_op = true; fir(x.d, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, u.d, 1.f, /*box=*/true); tan_op = false; }
+    twin([&](bool d) { fir(d ? x.d : x.p, B, H, H, x.C, 2, 1, 1, 0, m.tc0 ? om : 0, d ? u.d : u.p, 1.f, /*box=*/true); });
     Tensor out = talloc(m.cout, Ho, Ho);
-    conv(m.tc0, u, Tensor(), 9, m.w, m.b, m.cout, -1, nullptr, 1.f, 0, out, /*want_stats=*/true);
-    conv_t(m.tc0, u, Tensor(), 9, m.w, m.cout, nullptr, 1.f, 0, out);
+    conv(m.tc0, u, Tensor(), m.w, m.b, out, Conv().stats());
     tfree(u);
     return out;
   }
 
-  int build() {
+  // ---- time embedding (ncsnpp.py:236-255) + all Dense_0(act(temb)) rows (layerspp.py:263) ----
+  void time_embedding() {
     const b200_ncsnpp_config& c = e->cfg;
-    const int nf = c.nf, R = c.image_size, ch = c.num_channels, sumC = e->sumC;
+    const int nf = c.nf, sumC = e->sumC, Bc = B, ln = lane;
     b200_ncsnpp* eng = e;
-    const int Bc = B;
-    const int ln = lane;
-    // ---- time embedding (ncsnpp.py:236-255) + all Dense_0(act(temb)) rows (layerspp.py:263) ----
-    long long eb, t1b, t2b, db, xcb;
+    long long eb, t1b, t2b, db;
     const int positional = c.embedding_type == 1 ? 1 : 0, emb_dim = positional ? nf : 2 * nf;
     float* emb = falloc((long long)B * 2 * nf, &eb);
     float* t1 = falloc((long long)B * 4 * nf, &t1b);
     float* t2 = falloc((long long)B * 4 * nf, &t2b);
     float* dense_all = falloc((long long)B * sumC, &db);
     dense_all_ = dense_all;
-    {
-      const Mod &mf = e->mods[0], &l1 = e->mods[1], &l2 = e->mods[2];
-      const float *Wf = e->W(mf.w), *W1 = e->W(l1.w), *b1 = e->W(l1.b), *W2 = e->W(l2.w), *b2 = e->W(l2.b);
-      const float *Wd = e->wblob + e->dense_w_off, *bd = e->wblob + e->dense_b_off;
-      op(4, [=](cudaStream_t st) {
-        const int rows = eng->uniform ? 1 : Bc;
-        if (int r = launch_fourier_embed(eng->in_labels_l[ln], 1, Wf, positional ? nf / 2 : nf, rows, emb, st, positional)) return r;
-        if (int r = launch_linear_rows(emb, emb_dim, W1, b1, rows, 4 * nf, emb_dim, 0, t1, 4 * nf, st)) return r;
-        if (int r = launch_linear_rows(t1, 4 * nf, W2, b2, rows, 4 * nf, 4 * nf, 1, t2, 4 * nf, st)) return r;
-        return launch_linear_rows(t2, 4 * nf, Wd, bd, rows, sumC, 4 * nf, 1, dense_all, sumC, st);
-      }, 5);
-    }
-    // ---- input (ncsnpp.py:259-268) ----
-    float* dxc = nullptr;   // its tangent: v, or 2v (tangent plans)
-    float* xc = falloc2((long long)B * ch * R * R, &xcb, &dxc);   // 2x-1 when data is not centred; NCHW
-    {
-      const long long n = (long long)B * ch * R * R;
-      const int centered = c.centered;
+    const Mod &mf = e->mods[0], &l1 = e->mods[1], &l2 = e->mods[2];
+    const float *Wf = e->W(mf.w), *W1 = e->W(l1.w), *b1 = e->W(l1.b), *W2 = e->W(l2.w), *b2 = e->W(l2.b);
+    const float *Wd = e->wblob + e->dense_w_off, *bd = e->wblob + e->dense_b_off;
+    op(4, [=](cudaStream_t st) {
+      const int rows = eng->uniform ? 1 : Bc;
+      if (int r = launch_fourier_embed(eng->in_labels_l[ln], 1, Wf, positional ? nf / 2 : nf, rows, emb, st, positional)) return r;
+      if (int r = launch_linear_rows(emb, emb_dim, W1, b1, rows, 4 * nf, emb_dim, 0, t1, 4 * nf, st)) return r;
+      if (int r = launch_linear_rows(t1, 4 * nf, W2, b2, rows, 4 * nf, 4 * nf, 1, t2, 4 * nf, st)) return r;
+      return launch_linear_rows(t2, 4 * nf, Wd, bd, rows, sumC, 4 * nf, 1, dense_all, sumC, st);
+    }, 5);
+  }
+
+  // ---- input (ncsnpp.py:259-268): 2x-1 when the data is not centred (its tangent: v, or 2v), NCHW; then the input conv.
+  // The input also is the bottom of the input pyramid. ----
+  Tensor input_conv() {
+    const b200_ncsnpp_config& c = e->cfg;
+    const int nf = c.nf, R = c.image_size, ch = c.num_channels, ln = lane, centered = c.centered;
+    b200_ncsnpp* eng = e;
+    const Mod& m = next();
+    long long xcb; float* dxc = nullptr;
+    float* xc = falloc2((long long)B * ch * R * R, &xcb, &dxc);
+    const long long n = (long long)B * ch * R * R;
+    twin([&](bool d) {
+      float* dst = d ? dxc : xc;
+      const float shift = d ? 0.0f : -0.5f;
       op(1, [=](cudaStream_t st) {
-        if (centered) return cudaMemcpyAsync(xc, eng->in_x_l[ln], n * 4, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : (set_error("memcpy failed"), 1);
-        launch_kernel(affine_kernel, dim3((int)std::min<long long>((n + 255) / 256, 4096)), dim3(256), 0, st, eng->in_x_l[ln], xc, n, -0.5f, 2.0f);
+        const float* src = d ? eng->in_v : eng->in_x_l[ln];
+        if (centered) return cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : (set_error("memcpy failed"), 1);
+        launch_kernel(affine_kernel, dim3((int)std::min<long long>((n + 255) / 256, 4096)), dim3(256), 0, st, src, dst, n, shift, 2.0f);
         return cudaGetLastError() == cudaSuccess ? 0 : (set_error("affine launch failed"), 1);
       });
-      if (tan) {
-        tan_op = true;
-        op(1, [=](cudaStream_t st) {
-          if (centered) return cudaMemcpyAsync(dxc, eng->in_v, n * 4, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : (set_error("memcpy failed"), 1);
-          launch_kernel(affine_kernel, dim3((int)std::min<long long>((n + 255) / 256, 4096)), dim3(256), 0, st, eng->in_v, dxc, n, 0.0f, 2.0f);
-          return cudaGetLastError() == cudaSuccess ? 0 : (set_error("affine launch failed"), 1);
-        });
-        tan_op = false;
-      }
-    }
-    size_t mi = 3;
-    std::vector<Tensor> hs;
-    {
-      const Mod& m = e->mods[mi++];
-      Tensor h0 = talloc(nf, R, R);
-      if (m.tc0 || m.tc1) {
-        // im2col patches [B*R*R][32] (TF32 grid) then one K=32 contraction with the flat-packed weights (tensor cores, or the
-        // few-channel kernel for nf <= 64)
-        float* dpatches = nullptr;
-        long long pb; float* patches = falloc2((long long)B * R * R * 32, &pb, &dpatches);   // 128 B per pixel: 32 fp32 or 64 fp16
-        const int Bc = B, omc = om;
+    });
+    pyr.p = xc; pyr.C = ch; pyr.H = R; pyr.W = R;
+    Tensor h0 = talloc(nf, R, R);
+    if (m.tc0 || m.tc1) {
+      // im2col patches [B*R*R][32] (TF32 grid) then one K=32 contraction with the flat-packed weights (tensor cores, or the
+      // few-channel kernel for nf <= 64)
+      float* dpatches = nullptr;
+      long long pb; float* patches = falloc2((long long)B * R * R * 32, &pb, &dpatches);   // 128 B per pixel: 32 fp32 or 64 fp16
+      const int Bc = B, omc = om;
+      twin([&](bool d) {
+        const float* src = d ? dxc : xc; float* dst = d ? dpatches : patches;
         name("im2col 3x3 %d @%d", ch, R);
-        op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(xc, patches, Bc, ch, R, R, R, R, 1, 1, omc, st); }, 6);
-        if (tan) {
-          name("im2col 3x3 %d @%d", ch, R);
-          tan_op = true;
-          op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(dxc, dpatches, Bc, ch, R, R, R, R, 1, 1, omc, st); }, 6);
-          tan_op = false;
-        }
-        Tensor pt; pt.p = patches; pt.C = om == 2 ? 64 : 32; pt.H = R; pt.W = R;   // patches as a one-K-step NHWC image: a 1x1 conv
-        pt.d = dpatches;
-        conv(m.tc0, pt, Tensor(), 1, m.w, m.b, nf, -1, nullptr, 1.f, 0, h0, /*want_stats=*/true);
-        conv_t(m.tc0, pt, Tensor(), 1, m.w, nf, nullptr, 1.f, 0, h0);
-        ffree(patches, pb);
-      } else {
-        SimtConv s; memset(&s, 0, sizeof(s));
-        s.x1 = xc; s.C1 = ch; s.in_nchw = 1; s.in_scale = 1.f; s.H = R; s.W = R; s.R = s.S = 3; s.stride = 1; s.pad = 1;
-        s.OH = R; s.OW = R; s.nbatch = B; s.a_batched = 1; s.w = e->W(m.w); s.N = nf;
-        s.epi.bias = e->W(m.b); s.epi.scale = 1.f; s.epi.rows_per_img = R * R; s.epi.out = h0.p; s.epi.ld_out = nf;
+        op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(src, dst, Bc, ch, R, R, R, R, 1, 1, omc, st); }, 6);
+      });
+      Tensor pt; pt.p = patches; pt.C = om == 2 ? 64 : 32; pt.H = R; pt.W = R;   // patches as a one-K-step NHWC image: a 1x1 conv
+      pt.d = dpatches;
+      conv(m.tc0, pt, Tensor(), m.w, m.b, h0, Conv().taps(1).stats());
+      ffree(patches, pb);
+    } else {
+      twin([&](bool d) {
+        SimtConv s = simt_desc(d ? dxc : xc, ch, R, R, 9, 1, R, R, e->W(m.w), nf);
+        s.in_nchw = 1; s.epi.bias = d ? nullptr : e->W(m.b); s.epi.out = d ? h0.d : h0.p;
         op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * R * R * (double)nf * ch * 9);
-        if (tan) {
-          SimtConv sd = s; sd.x1 = dxc; sd.epi.bias = nullptr; sd.epi.out = h0.d;
-          tan_op = true;
-          op(1, [=](cudaStream_t st) { return launch_conv_simt(sd, st); }, 1, 2.0 * B * R * R * (double)nf * ch * 9);
-          tan_op = false;
-        }
-      }
-      hs.push_back(h0);
-      tap(m.index, h0);
+      });
     }
-    // input pyramid (progressive_input='residual', ncsnpp.py:289-301): starts as the network input
-    Tensor pyr; pyr.p = xc; pyr.C = ch; pyr.H = R; pyr.W = R; bool pyr_nchw = true; bool pyr_owned = false; long long pyr_bytes = 0;
+    tap(m.index, h0);
+    return h0;
+  }
+
+  // ---- one level of the input pyramid (ncsnpp.py:289-301), after the level's downsampling block h ----
+  Tensor input_pyramid(Tensor h) {
+    const b200_ncsnpp_config& c = e->cfg;
+    const int ch = c.num_channels;
+    const Mod& m = next();
+    if (m.kind == M_COMBINE) {
+      // input_skip (ncsnpp.py:289-292): the image pyramid is downsampled (no parameters) and a 1x1 convolution of it is
+      // added to h: Combine(method='sum') (layerspp.py:44-59)
+      const int Hin = pyr.H, Hn = Hin / 2;
+      long long nb; float* npyr = falloc((long long)B * ch * Hn * Hn, &nb);
+      resample2x_planes(pyr.p, B * ch, Hin, false, npyr);
+      if (pyr_owned) ffree(pyr.p, pyr_bytes);
+      pyr.p = npyr; pyr.H = pyr.W = Hn; pyr_owned = true; pyr_bytes = nb;
+      if (Hn != h.H) { set_error("ncsnpp: input pyramid geometry mismatch (%d vs %d)", Hn, h.H); rc = 2; return Tensor(); }
+      Tensor out = talloc(m.cout, h.H, h.W);
+      SimtConv s = simt_desc(npyr, ch, Hn, Hn, 1, 1, Hn, Hn, e->W(m.w), m.cout);
+      s.in_nchw = 1; s.epi.bias = e->W(m.b); s.epi.residual = h.p; s.epi.out = out.p;
+      name("combine sum: conv1x1 %d->%d @%d +h [cuda-core]", ch, m.cout, Hn);
+      op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * Hn * Hn * (double)m.cout * ch);
+      advance(h, m, out);
+      return h;
+    }
+    // residual (M_PYR_DOWN): Downsample(fir, with_conv): FIR with pad (2,2) then 3x3 stride-2 VALID conv + bias
+    // (up_or_down_sampling.py:170-178, Conv2d.forward :44-56), then (pyr + h)/sqrt2 (ncsnpp.py:297-301)
+    const int Hin = pyr.H, p = (e->firn - 2) + 2;
+    const int Hp = Hin + ((p + 1) / 2) + (p / 2) - e->firn + 1;
+    long long fb; float* fbuf = falloc((long long)B * pyr.C * Hp * Hp, &fb);
+    const bool tcp = m.tc0 && !pyr_nchw;
+    const bool flat = m.tc2 && pyr_nchw;
+    if (pyr_nchw) fir(pyr.p, B * pyr.C, Hin, Hin, 1, 1, 1, (p + 1) / 2, p / 2, 0, fbuf, 1.f);
+    else fir(pyr.p, B, Hin, Hin, pyr.C, 1, 1, (p + 1) / 2, p / 2, tcp ? om : 0, fbuf, 1.f);
+    Tensor np = talloc(m.cout, h.H, h.W);
+    if ((Hp - 3) / 2 + 1 != h.H) { set_error("ncsnpp: pyramid geometry mismatch (%d vs %d)", (Hp - 3) / 2 + 1, h.H); rc = 2; return Tensor(); }
+    const float ps = c.skip_rescale ? 1.0f / (float)std::sqrt(2.0) : 1.0f;
+    if (flat) {
+      long long pb2; float* patches = falloc((long long)B * h.H * h.W * 32, &pb2);
+      const int Bc = B, pc = pyr.C, oh = h.H, ow = h.W, omc = om;
+      name("im2col 3x3 s2 %d @%d", pc, oh);
+      op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(fbuf, patches, Bc, pc, Hp, Hp, oh, ow, 2, 0, omc, st); }, 6);
+      Tensor pt; pt.p = patches; pt.C = om == 2 ? 64 : 32; pt.H = h.H; pt.W = h.W;
+      conv(true, pt, Tensor(), m.w, m.b, np, Conv().taps(1).residual(h).scale(ps).stats());
+      ffree(patches, pb2);
+    } else if (tcp) {
+      Tensor fin; fin.p = fbuf; fin.C = pyr.C; fin.H = Hp; fin.W = Hp;
+      conv(true, fin, Tensor(), m.w, m.b, np, Conv().residual(h).scale(ps).stats().stride(2, Hp));
+    } else {
+      SimtConv s = simt_desc(fbuf, pyr.C, Hp, Hp, 9, 2, h.H, h.W, e->W(m.w), m.cout);
+      s.in_nchw = pyr_nchw ? 1 : 0; s.epi.bias = e->W(m.b); s.epi.residual = h.p; s.epi.scale = ps; s.epi.out = np.p;
+      op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * h.H * h.W * (double)m.cout * pyr.C * 9);
+    }
+    ffree(fbuf, fb);
+    if (pyr_owned) tfree(pyr);
+    tfree(h);
+    pyr = np; pyr_nchw = false; pyr_owned = false;   // h aliases the pyramid from here on (it lives in hs)
+    // (no debug tap: the reference module's own output is the pre-combine conv result, which is never materialised)
+    return np;
+  }
+
+  // ---- middle (ncsnpp.py:305-311): resblock, attention, resblock ----
+  Tensor middle(Tensor& x) {
+    Tensor none;
+    const Mod& m0 = next(); Tensor h = resblock(m0, x, none); if (rc) return h;
+    tap(m0.index, h);
+    const Mod& ma = next(); Tensor h2 = attn(ma, h); if (rc) return h2;
+    advance(h, ma, h2);
+    const Mod& m1 = next(); Tensor h3 = resblock(m1, h, none); if (rc) return h3;
+    advance(h, m1, h3);
+    return h;
+  }
+
+  // ---- one output_skip level (ncsnpp.py:325-341): pyramid = upsample(pyramid) + conv3x3(SiLU(GroupNorm(h))) in image
+  // channels; the level-0 sum is the network output (divided by sigma when scale_by_sigma, :377-379) ----
+  void output_skip(Tensor& h, bool last) {
+    const b200_ncsnpp_config& c = e->cfg;
+    const int ch = c.num_channels, Hl = h.H, ln = lane;
+    b200_ncsnpp* eng = e;
+    const Mod& mg = next(); const Mod& mo = next();
+    Tensor a = talloc(h.C, Hl, Hl);
+    const int hf16 = (om == 2 && h.C % 64 == 0) ? 1 : 0;
+    Tensor none; gn(h, none, mg.w, mg.b, 1, hf16 ? 2 : 0, a, nullptr);
+    long long ub = 0; float* up = nullptr;
+    if (opyr) {
+      up = falloc((long long)B * ch * Hl * Hl, &ub);
+      resample2x_planes(opyr, B * ch, Hl / 2, true, up);
+      ffree(opyr, opyr_bytes); opyr = nullptr;
+    }
+    long long nb = 0; float* dst = nullptr;
+    if (!last) dst = falloc((long long)B * ch * Hl * Hl, &nb);
+    const float *wo = e->W(mo.w), *bo = e->W(mo.b);
+    const Tensor ain = a; const int Bc2 = B, sbs = c.scale_by_sigma;
+    if (ch > 4) { set_error("ncsnpp: output_skip needs <= 4 image channels"); rc = 2; return; }
+    name("conv3x3 %d->%d @%d nchw-out +pyramid [small-n]", a.C, ch, Hl);
+    op(1, [=](cudaStream_t st) {
+      return launch_conv3x3_small_n(ain.p, wo, bo, (last && sbs) ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1,
+                                    last ? eng->out_l[ln] : dst, Bc2, Hl, Hl, ain.C, ch, hf16, st, up);
+    }, 1, 2.0 * B * Hl * Hl * (double)ch * a.C * 9);
+    tfree(a);
+    if (up) ffree(up, ub);
+    opyr = dst; opyr_bytes = nb;
+  }
+
+  // ---- output head (ncsnpp.py:371-379): GroupNorm, SiLU, 3x3 conv to the image channels, stored NCHW, / sigma.  Its
+  // tangent writes J v into tout. ----
+  void head(Tensor& h) {
+    const b200_ncsnpp_config& c = e->cfg;
+    const int R = c.image_size, ch = c.num_channels, ln = lane, Bc = B, sbs = c.scale_by_sigma;
+    b200_ncsnpp* eng = e;
+    const Mod& mg = next(); const Mod& mo = next();
+    Tensor a = talloc(h.C, h.H, h.W);
+    // fp16 operand mode: the head's input is stored as fp16 too (the CUDA-core head is bound by its nine-fold
+    // tap re-reads through L1/L2, so half the bytes is half the time); same 11-bit rounding as every other conv input
+    const int head_f16 = (!mo.tc0 && om == 2 && ch <= 4 && h.C % 64 == 0) ? 1 : 0;
+    Tensor none; gn(h, none, mg.w, mg.b, 1, mo.tc0 ? om : head_f16 ? 2 : 0, a, nullptr);
+    tfree(h);
+    const float *wo = e->W(mo.w), *bo = e->W(mo.b);
+    const double flops = 2.0 * B * R * R * (double)ch * a.C * 9;
+    twin([&](bool d) {
+      const float* x = d ? a.d : a.p;
+      const float* bias = d ? nullptr : bo;
+      if (mo.tc0) {
+        if (dry) return;
+        TcGemmDesc desc = tc_desc(e, x, a.C, nullptr, 0, R, R, B, 9, wo, 128);
+        desc.stride = 1;
+        desc.epi.bias = bias; desc.epi.scale = 1.f; desc.epi.rows_per_img = R * R; desc.epi.out_nchw = 1; desc.epi.n_valid = ch;
+        desc.epi.out = reinterpret_cast<float*>(uintptr_t(16));   // patched per call (tc_gemm_set_head)
+        TcGemmPlan* pl = nullptr;
+        if (int r = tc_gemm_plan_create(desc, &pl)) { rc = r; return; }
+        e->tcplans.push_back(pl);
+        name("conv3x3 %d->%d(pad 128) @%d nchw-out /sigma [%s]", a.C, ch, R, tc_gemm_form(pl));
+        next_bytes = (double)B * R * R * (a.C * (om == 2 ? 2.0 : 4.0) + ch * 4.0);
+        op(1, [=](cudaStream_t st) {
+          tc_gemm_set_head(pl, d ? eng->tout : eng->out_l[ln], sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1);
+          return tc_gemm_launch(pl, st);
+        }, 0, flops);
+      } else if (ch <= 4) {
+        const int C = a.C;
+        name("conv3x3 %d->%d @%d nchw-out [small-n]", C, ch, R);
+        op(1, [=](cudaStream_t st) {
+          return launch_conv3x3_small_n(x, wo, bias, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1,
+                                        d ? eng->tout : eng->out_l[ln], Bc, R, R, C, ch, head_f16, st);
+        }, 1, flops);
+      } else {
+        SimtConv s = simt_desc(x, a.C, R, R, 9, 1, R, R, wo, ch);
+        s.epi.bias = bias; s.epi.out_nchw = 1;
+        op(1, [=](cudaStream_t st) {
+          SimtConv cc = s;
+          cc.epi.out = d ? eng->tout : eng->out_l[ln];
+          if (sbs) { cc.epi.per_img_div = eng->in_labels_l[ln]; cc.epi.div_stride = eng->uniform ? 0 : 1; }
+          return launch_conv_simt(cc, st);
+        }, 1, flops);
+      }
+    });
+    tfree(a);
+  }
+
+  // the forward pass (models/ncsnpp.py:232-381) as a walk over e->mods
+  int build() {
+    const b200_ncsnpp_config& c = e->cfg;
     const int L = c.num_levels;
+    Tensor none;
+    time_embedding();
+    std::vector<Tensor> hs = {input_conv()};
     for (int lvl = 0; lvl < L; ++lvl) {
       for (int b = 0; b < c.num_res_blocks; ++b) {
-        const Mod& m = e->mods[mi++];
-        Tensor none; Tensor h = resblock(m, hs.back(), none); if (rc) return rc;
+        const Mod& m = next();
+        Tensor h = resblock(m, hs.back(), none); if (rc) return rc;
         tap(m.index, h);
-        if (mi < e->mods.size() && e->mods[mi].kind == M_ATTN && e->mods[mi].res == h.H && lvl_has_attn(h.H)) {
-          const Mod& ma = e->mods[mi++];
+        if (mi < e->mods.size() && e->mods[mi].kind == M_ATTN && e->mods[mi].res == h.H && has_attn(c, h.H)) {
+          const Mod& ma = next();
           Tensor h2 = attn(ma, h); if (rc) return rc;
-          tfree(h); h = h2; tap(ma.index, h);
+          advance(h, ma, h2);
         }
         hs.push_back(h);
       }
       if (lvl != L - 1) {
-        const Mod& m = e->mods[mi++];
-        Tensor none; Tensor h = m.kind == M_DOWN ? downsample(m, hs.back()) : resblock(m, hs.back(), none); if (rc) return rc;
+        const Mod& m = next();
+        Tensor h = m.kind == M_DOWN ? downsample(m, hs.back()) : resblock(m, hs.back(), none); if (rc) return rc;
         tap(m.index, h);
-        if (c.progressive_input == 2) {
-          // input_skip (ncsnpp.py:289-292): the image pyramid is downsampled (no parameters) and a 1x1 convolution of it is
-          // added to h: Combine(method='sum') (layerspp.py:44-59)
-          const Mod& mc = e->mods[mi++];
-          const int Hin = pyr.H, Hn = Hin / 2;
-          long long nb; float* npyr = falloc((long long)B * ch * Hn * Hn, &nb);
-          resample2x_planes(pyr.p, B * ch, Hin, false, npyr);
-          if (pyr_owned) ffree(pyr.p, pyr_bytes);
-          pyr.p = npyr; pyr.H = pyr.W = Hn; pyr_owned = true; pyr_bytes = nb;
-          if (Hn != h.H) { set_error("ncsnpp: input pyramid geometry mismatch (%d vs %d)", Hn, h.H); return 2; }
-          Tensor out = talloc(mc.cout, h.H, h.W);
-          SimtConv sc; memset(&sc, 0, sizeof(sc));
-          sc.x1 = npyr; sc.C1 = ch; sc.in_nchw = 1; sc.in_scale = 1.f; sc.H = Hn; sc.W = Hn; sc.R = sc.S = 1; sc.stride = 1; sc.pad = 0;
-          sc.OH = Hn; sc.OW = Hn; sc.nbatch = B; sc.a_batched = 1; sc.w = e->W(mc.w); sc.N = mc.cout;
-          sc.epi.bias = e->W(mc.b); sc.epi.residual = h.p; sc.epi.ld_res = mc.cout; sc.epi.scale = 1.f;
-          sc.epi.rows_per_img = Hn * Hn; sc.epi.out = out.p; sc.epi.ld_out = mc.cout;
-          name("combine sum: conv1x1 %d->%d @%d +h [cuda-core]", ch, mc.cout, Hn);
-          op(1, [=](cudaStream_t st) { return launch_conv_simt(sc, st); }, 1, 2.0 * B * Hn * Hn * (double)mc.cout * ch);
-          tfree(h);
-          h = out; tap(mc.index, h);
-        }
-        if (c.progressive_input == 1) {
-          const Mod& mp = e->mods[mi++];
-          // Downsample(fir, with_conv): FIR with pad (2,2) then 3x3 stride-2 VALID conv + bias
-          // (up_or_down_sampling.py:170-178, Conv2d.forward :44-56), then (pyr + h)/sqrt2 (ncsnpp.py:297-301)
-          const int Hin = pyr.H, p = (e->firn - 2) + 2;
-          const int Hp = Hin + ((p + 1) / 2) + (p / 2) - e->firn + 1;
-          long long fb; float* fbuf = falloc((long long)B * pyr.C * Hp * Hp, &fb);
-          const bool tcp = mp.tc0 && !pyr_nchw;
-          const bool flat = mp.tc2 && pyr_nchw;
-          if (pyr_nchw) fir(pyr.p, B * pyr.C, Hin, Hin, 1, 1, 1, (p + 1) / 2, p / 2, 0, fbuf, 1.f);
-          else fir(pyr.p, B, Hin, Hin, pyr.C, 1, 1, (p + 1) / 2, p / 2, tcp ? om : 0, fbuf, 1.f);
-          Tensor np = talloc(mp.cout, h.H, h.W);
-          if ((Hp - 3) / 2 + 1 != h.H) { set_error("ncsnpp: pyramid geometry mismatch (%d vs %d)", (Hp - 3) / 2 + 1, h.H); return 2; }
-          const float ps = c.skip_rescale ? 1.0f / (float)std::sqrt(2.0) : 1.0f;
-          if (flat) {
-            long long pb2; float* patches = falloc((long long)B * h.H * h.W * 32, &pb2);
-            const int Bc = B, pc = pyr.C, oh = h.H, ow = h.W, omc = om;
-            name("im2col 3x3 s2 %d @%d", pc, oh);
-            op(1, [=](cudaStream_t st) { return launch_im2col3x3_nchw(fbuf, patches, Bc, pc, Hp, Hp, oh, ow, 2, 0, omc, st); }, 6);
-            Tensor pt; pt.p = patches; pt.C = om == 2 ? 64 : 32; pt.H = h.H; pt.W = h.W;
-            conv(true, pt, Tensor(), 1, mp.w, mp.b, mp.cout, -1, h.p, ps, 0, np, /*want_stats=*/true);
-            ffree(patches, pb2);
-          } else if (tcp) {
-            Tensor fin; fin.p = fbuf; fin.C = pyr.C; fin.H = Hp; fin.W = Hp;
-            conv(true, fin, Tensor(), 9, mp.w, mp.b, mp.cout, -1, h.p, ps, 0, np, /*want_stats=*/true, /*stride=*/2, /*Hin=*/Hp);
-          } else {
-            SimtConv s; memset(&s, 0, sizeof(s));
-            s.x1 = fbuf; s.C1 = pyr.C; s.in_nchw = pyr_nchw ? 1 : 0; s.in_scale = 1.f; s.H = Hp; s.W = Hp; s.R = s.S = 3; s.stride = 2; s.pad = 0;
-            s.OH = h.H; s.OW = h.W; s.nbatch = B; s.a_batched = 1; s.w = e->W(mp.w); s.N = mp.cout;
-            s.epi.bias = e->W(mp.b); s.epi.residual = h.p; s.epi.ld_res = mp.cout; s.epi.scale = ps;
-            s.epi.rows_per_img = h.H * h.W; s.epi.out = np.p; s.epi.ld_out = mp.cout;
-            op(1, [=](cudaStream_t st) { return launch_conv_simt(s, st); }, 1, 2.0 * B * h.H * h.W * (double)mp.cout * pyr.C * 9);
-          }
-          ffree(fbuf, fb);
-          if (pyr_owned) tfree(pyr);
-          tfree(h);
-          h = np; pyr = np; pyr_nchw = false; pyr_owned = false;   // h aliases the pyramid from here on (it lives in hs)
-          // (no debug tap: the reference module's own output is the pre-combine conv result, which is never materialised)
-        }
+        if (c.progressive_input) { h = input_pyramid(h); if (rc) return rc; }
         hs.push_back(h);
       }
     }
-    // ---- middle (ncsnpp.py:305-311) ----
-    Tensor h;
-    {
-      Tensor none; const Mod& m0 = e->mods[mi++]; h = resblock(m0, hs.back(), none); if (rc) return rc; tap(m0.index, h);
-      const Mod& ma = e->mods[mi++]; Tensor h2 = attn(ma, h); if (rc) return rc; tfree(h); h = h2; tap(ma.index, h);
-      const Mod& m1 = e->mods[mi++]; Tensor h3 = resblock(m1, h, none); if (rc) return rc; tfree(h); h = h3; tap(m1.index, h);
-    }
+    Tensor h = middle(hs.back()); if (rc) return rc;
     // ---- up path (ncsnpp.py:316-364) ----
-    float* opyr = nullptr; long long opyr_bytes = 0;      // output_skip pyramid [B][ch][H][W] of the previous (coarser) level
     for (int lvl = L - 1; lvl >= 0; --lvl) {
       for (int b = 0; b < c.num_res_blocks + 1; ++b) {
-        const Mod& m = e->mods[mi++];
+        const Mod& m = next();
         Tensor skip = hs.back(); hs.pop_back();
         Tensor h2 = resblock(m, h, skip); if (rc) return rc;
-        tfree(h); tfree(skip);
-        h = h2; tap(m.index, h);
+        advance(h, m, h2);
+        tfree(skip);
       }
       if (e->mods[mi].kind == M_ATTN) {
-        const Mod& ma = e->mods[mi++]; Tensor h2 = attn(ma, h); if (rc) return rc; tfree(h); h = h2; tap(ma.index, h);
+        const Mod& ma = next();
+        Tensor h2 = attn(ma, h); if (rc) return rc;
+        advance(h, ma, h2);
       }
-      if (c.progressive == 1) {
-        // output_skip (ncsnpp.py:325-341): pyramid = upsample(pyramid) + conv3x3(SiLU(GroupNorm(h))) in image channels;
-        // the level-0 sum is the network output (divided by sigma when scale_by_sigma, :377-379)
-        const Mod& mg = e->mods[mi++]; const Mod& mo = e->mods[mi++];
-        const int Hl = h.H;
-        Tensor a = talloc(h.C, Hl, Hl);
-        const int hf16 = (om == 2 && h.C % 64 == 0) ? 1 : 0;
-        Tensor none; gn(h, none, mg.w, mg.b, 1, hf16 ? 2 : 0, a, nullptr);
-        long long ub = 0; float* up = nullptr;
-        if (opyr) {
-          up = falloc((long long)B * ch * Hl * Hl, &ub);
-          resample2x_planes(opyr, B * ch, Hl / 2, true, up);
-          ffree(opyr, opyr_bytes); opyr = nullptr;
-        }
-        long long nb = 0; float* dst = nullptr;
-        if (lvl != 0) dst = falloc((long long)B * ch * Hl * Hl, &nb);
-        const float *wo = e->W(mo.w), *bo = e->W(mo.b);
-        const Tensor ain = a; const int Bc2 = B, sbs = c.scale_by_sigma, last = lvl == 0;
-        if (ch > 4) { set_error("ncsnpp: output_skip needs <= 4 image channels"); return 2; }
-        name("conv3x3 %d->%d @%d nchw-out +pyramid [small-n]", a.C, ch, Hl);
-        op(1, [=](cudaStream_t st) {
-          return launch_conv3x3_small_n(ain.p, wo, bo, (last && sbs) ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1,
-                                        last ? eng->out_l[ln] : dst, Bc2, Hl, Hl, ain.C, ch, hf16, st, up);
-        }, 1, 2.0 * B * Hl * Hl * (double)ch * a.C * 9);
-        tfree(a);
-        if (up) ffree(up, ub);
-        opyr = dst; opyr_bytes = nb;
-      }
+      if (c.progressive == 1) { output_skip(h, lvl == 0); if (rc) return rc; }
       if (lvl != 0) {
-        Tensor none; const Mod& m = e->mods[mi++];
+        const Mod& m = next();
         Tensor h2 = m.kind == M_UP ? upsample(m, h) : resblock(m, h, none); if (rc) return rc;
-        tfree(h); h = h2; tap(m.index, h);
+        advance(h, m, h2);
       }
     }
-    // ---- output head (ncsnpp.py:371-379); with output_skip the pyramid already is the output ----
-    if (c.progressive != 1) {
-      const Mod& mg = e->mods[mi++];
-      Tensor a = talloc(h.C, h.H, h.W);
-      // fp16 operand mode: the head's input is stored as fp16 too (the CUDA-core head is bound by its nine-fold
-      // tap re-reads through L1/L2, so half the bytes is half the time); same 11-bit rounding as every other conv input
-      const Mod& mo = e->mods[mi];
-      const int head_f16 = (!mo.tc0 && om == 2 && ch <= 4 && h.C % 64 == 0) ? 1 : 0;
-      Tensor none; gn(h, none, mg.w, mg.b, 1, mo.tc0 ? om : head_f16 ? 2 : 0, a, nullptr);
-      tfree(h);
-      ++mi;
-      const int sbs = c.scale_by_sigma;
-      const float *wo = e->W(mo.w), *bo = e->W(mo.b);
-      const Tensor ain = a; const int Bc = B;
-      if (mo.tc0) {
-        TcGemmDesc d; memset(&d, 0, sizeof(d));
-        d.a1 = a.p; d.C1 = a.C; d.conv = 1; d.H = R; d.W = R; d.nimg = B; d.taps = 9; d.stride = 1;
-        d.w = wo; d.N_total = 128; d.K_total = a.C; d.w_rows = 9LL * 128; d.nbatch = 1; d.f16 = om == 2; d.no_halo = e->cfg.no_halo;
-        d.epi.bias = bo; d.epi.scale = 1.f; d.epi.rows_per_img = R * R; d.epi.out_nchw = 1; d.epi.n_valid = ch; d.epi.ld_out = 128;
-        d.epi.out = reinterpret_cast<float*>(uintptr_t(16));   // patched per call (tc_gemm_set_head)
-        if (!dry) {
-          TcGemmPlan* pl = nullptr;
-          if (int r = tc_gemm_plan_create(d, &pl)) { rc = r; return r; }
-          e->tcplans.push_back(pl);
-          name("conv3x3 %d->%d(pad 128) @%d nchw-out /sigma [%s]", a.C, ch, R, tc_gemm_form(pl));
-          next_bytes = (double)B * R * R * (a.C * (om == 2 ? 2.0 : 4.0) + ch * 4.0);
-          op(1, [=](cudaStream_t st) {
-            tc_gemm_set_head(pl, eng->out_l[ln], sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1);
-            return tc_gemm_launch(pl, st);
-          }, 0, 2.0 * B * R * R * (double)ch * a.C * 9);
-          if (tan) {   // J v: the same head over the tangent, without bias, into the jvp output
-            TcGemmDesc dd = d; dd.a1 = a.d; dd.epi.bias = nullptr;
-            TcGemmPlan* pt = nullptr;
-            if (int r = tc_gemm_plan_create(dd, &pt)) { rc = r; return r; }
-            e->tcplans.push_back(pt);
-            name("conv3x3 %d->%d(pad 128) @%d nchw-out /sigma [%s]", a.C, ch, R, tc_gemm_form(pt));
-            tan_op = true;
-            op(1, [=](cudaStream_t st) {
-              tc_gemm_set_head(pt, eng->tout, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1);
-              return tc_gemm_launch(pt, st);
-            }, 0, 2.0 * B * R * R * (double)ch * a.C * 9);
-            tan_op = false;
-          }
-        }
-      } else if (ch <= 4) {
-        name("conv3x3 %d->%d @%d nchw-out [small-n]", a.C, ch, R);
-        op(1, [=](cudaStream_t st) {
-          return launch_conv3x3_small_n(ain.p, wo, bo, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1, eng->out_l[ln],
-                                        Bc, R, R, ain.C, ch, head_f16, st);
-        }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
-        if (tan) {
-          name("conv3x3 %d->%d @%d nchw-out [small-n]", a.C, ch, R);
-          tan_op = true;
-          op(1, [=](cudaStream_t st) {
-            return launch_conv3x3_small_n(ain.d, wo, nullptr, sbs ? eng->in_labels_l[ln] : nullptr, eng->uniform ? 0 : 1, eng->tout,
-                                          Bc, R, R, ain.C, ch, head_f16, st);
-          }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
-          tan_op = false;
-        }
-      } else {
-        SimtConv s; memset(&s, 0, sizeof(s));
-        s.x1 = a.p; s.C1 = a.C; s.in_scale = 1.f; s.H = R; s.W = R; s.R = s.S = 3; s.stride = 1; s.pad = 1;
-        s.OH = R; s.OW = R; s.nbatch = B; s.a_batched = 1; s.w = wo; s.N = ch;
-        s.epi.bias = bo; s.epi.scale = 1.f; s.epi.rows_per_img = R * R; s.epi.out_nchw = 1; s.epi.ld_out = ch;
-        op(1, [=](cudaStream_t st) {
-          SimtConv cc = s;
-          cc.epi.out = eng->out_l[ln];
-          if (sbs) { cc.epi.per_img_div = eng->in_labels_l[ln]; cc.epi.div_stride = eng->uniform ? 0 : 1; }
-          return launch_conv_simt(cc, st);
-        }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
-        if (tan) {
-          SimtConv sd = s; sd.x1 = a.d; sd.epi.bias = nullptr;
-          tan_op = true;
-          op(1, [=](cudaStream_t st) {
-            SimtConv cc = sd;
-            cc.epi.out = eng->tout;
-            if (sbs) { cc.epi.per_img_div = eng->in_labels_l[ln]; cc.epi.div_stride = eng->uniform ? 0 : 1; }
-            return launch_conv_simt(cc, st);
-          }, 1, 2.0 * B * R * R * (double)ch * a.C * 9);
-          tan_op = false;
-        }
-      }
-      tfree(a);
-    }
+    // with output_skip the pyramid already is the output
+    if (c.progressive != 1) { head(h); if (rc) return rc; }
     if (mi != e->mods.size()) { set_error("ncsnpp: plan walked %zu of %zu modules", mi, e->mods.size()); return 2; }
     if (!dry && stats_top > 0) {
       // the epilogue-accumulated GroupNorm sums start from zero every forward: one memset of the whole region
@@ -1261,13 +1247,7 @@ struct Builder {
         return cudaMemsetAsync(sb, 0, (size_t)sn, st) == cudaSuccess ? 0 : (set_error("stats memset failed"), 1);
       }, "zero GroupNorm sums", 0.0});
     }
-    (void)eb; (void)t1b; (void)t2b; (void)db; (void)xcb;
     return rc;
-  }
-
-  bool lvl_has_attn(int r) const {
-    for (int i = 0; i < e->cfg.num_attn_resolutions; ++i) if (e->cfg.attn_resolutions[i] == r) return true;
-    return false;
   }
 };
 
@@ -1427,6 +1407,35 @@ void set_call_args(b200_ncsnpp* h, const float* x, const float* labels, int unif
   h->in_x_l[0] = x; h->in_labels_l[0] = labels; h->out_l[0] = out;
   h->in_x_l[1] = x + h->B0 * per_img; h->in_labels_l[1] = uniform ? labels : labels + h->B0; h->out_l[1] = out + h->B0 * per_img;
 }
+
+// op i of the plan: lane 0's ops, then lane 1's; nullptr when out of range
+const b200_ncsnpp::Op* op_at(const b200_ncsnpp* h, long long i) {
+  if (!h || i < 0) return nullptr;
+  const long long n0 = (long long)h->ops.size();
+  if (i < n0) return &h->ops[i];
+  return i - n0 < (long long)h->ops2.size() ? &h->ops2[i - n0] : nullptr;
+}
+
+// every op of both lanes serially on ONE stream, each between two events: each launch is timed alone (no overlap), which is
+// what a per-kernel roofline needs.  ms[i] receives op i's time.
+int time_ops(b200_ncsnpp* h, const float* x, const float* labels, int uniform, float* out, void* stream, float* ms, const char* who) {
+  set_call_args(h, x, labels, uniform, out);
+  h->in_v = x; h->tout = out;   // tangent plans: the JVP pass along v = x
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const long long n = (long long)(h->ops.size() + h->ops2.size());
+  std::vector<cudaEvent_t> ev(n + 1);
+  for (auto& e : ev) B200_CHECK_CUDA(cudaEventCreate(&e));
+  int rc = 0;
+  B200_CHECK_CUDA(cudaEventRecord(ev[0], st));
+  for (long long i = 0; i < n && !rc; ++i) {
+    rc = op_at(h, i)->fn(st);
+    cudaEventRecord(ev[i + 1], st);
+  }
+  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { set_error("%s: stream sync failed", who); rc = 1; }
+  if (!rc) for (long long i = 0; i < n; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+  for (auto& e : ev) cudaEventDestroy(e);
+  return rc;
+}
 }  // namespace
 
 int b200_ncsnpp_forward(b200_ncsnpp_t* h, const float* x, const float* labels, int uniform, float* out, void* stream) {
@@ -1475,51 +1484,34 @@ int b200_ncsnpp_profile_forward(b200_ncsnpp_t* h, const float* x, const float* l
                                 void* stream, float ms_by_kind[8], double flops_by_kind[8], long long ops_by_kind[8]) {
   B200_REQUIRE(h && x && labels && out && ms_by_kind, "profile_forward: null argument");
   B200_REQUIRE(!h->ops.empty(), "profile_forward: no plan bound");
-  set_call_args(h, x, labels, uniform, out);
-  h->in_v = x; h->tout = out;   // tangent plans: the JVP pass along v = x
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   for (int k = 0; k < 8; ++k) { ms_by_kind[k] = 0.f; if (flops_by_kind) flops_by_kind[k] = 0.0; if (ops_by_kind) ops_by_kind[k] = 0; }
-  // both lanes serially on ONE stream: each launch is timed alone (no overlap), which is what a per-kernel roofline needs
-  std::vector<const b200_ncsnpp::Op*> all;
-  for (auto& o : h->ops) all.push_back(&o);
-  for (auto& o : h->ops2) all.push_back(&o);
-  std::vector<cudaEvent_t> ev(all.size() + 1);
-  for (auto& e : ev) B200_CHECK_CUDA(cudaEventCreate(&e));
-  int rc = 0;
-  B200_CHECK_CUDA(cudaEventRecord(ev[0], st));
-  for (size_t i = 0; i < all.size() && !rc; ++i) {
-    rc = all[i]->fn(st);
-    cudaEventRecord(ev[i + 1], st);
+  std::vector<float> ms(h->ops.size() + h->ops2.size());
+  if (int rc = time_ops(h, x, labels, uniform, out, stream, ms.data(), "profile_forward")) return rc;
+  for (size_t i = 0; i < ms.size(); ++i) {
+    const b200_ncsnpp::Op& o = *op_at(h, (long long)i);
+    const int k = o.kind & 7;
+    ms_by_kind[k] += ms[i];
+    if (flops_by_kind) flops_by_kind[k] += o.flops;
+    if (ops_by_kind) ops_by_kind[k] += 1;
   }
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { set_error("profile_forward: stream sync failed"); rc = 1; }
-  if (!rc) {
-    for (size_t i = 0; i < all.size(); ++i) {
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-      const int k = all[i]->kind & 7;
-      ms_by_kind[k] += ms;
-      if (flops_by_kind) flops_by_kind[k] += all[i]->flops;
-      if (ops_by_kind) ops_by_kind[k] += 1;
-    }
-  }
-  for (auto& e : ev) cudaEventDestroy(e);
-  return rc;
+  return 0;
 }
 
 long long b200_ncsnpp_num_ops(const b200_ncsnpp_t* h) { return h ? (long long)(h->ops.size() + h->ops2.size()) : 0; }
 
 int b200_ncsnpp_op_info(const b200_ncsnpp_t* h, long long index, char* name, int name_cap, int* kind, double* flops) {
-  B200_REQUIRE(h && index >= 0 && index < (long long)(h->ops.size() + h->ops2.size()), "op_info: index out of range");
-  const b200_ncsnpp::Op& o = index < (long long)h->ops.size() ? h->ops[index] : h->ops2[index - h->ops.size()];
-  if (name && name_cap > 0) { strncpy(name, o.name.c_str(), name_cap - 1); name[name_cap - 1] = 0; }
-  if (kind) *kind = o.kind;
-  if (flops) *flops = o.flops;
+  const b200_ncsnpp::Op* o = op_at(h, index);
+  B200_REQUIRE(o, "op_info: index out of range");
+  if (name && name_cap > 0) { strncpy(name, o->name.c_str(), name_cap - 1); name[name_cap - 1] = 0; }
+  if (kind) *kind = o->kind;
+  if (flops) *flops = o->flops;
   return 0;
 }
 
 int b200_ncsnpp_op_bytes(const b200_ncsnpp_t* h, long long index, double* bytes) {
-  B200_REQUIRE(h && bytes && index >= 0 && index < (long long)(h->ops.size() + h->ops2.size()), "op_bytes: index out of range");
-  *bytes = (index < (long long)h->ops.size() ? h->ops[index] : h->ops2[index - h->ops.size()]).bytes;
+  const b200_ncsnpp::Op* o = op_at(h, index);
+  B200_REQUIRE(o && bytes, "op_bytes: index out of range");
+  *bytes = o->bytes;
   return 0;
 }
 
@@ -1529,21 +1521,7 @@ int b200_ncsnpp_profile_ops(b200_ncsnpp_t* h, const float* x, const float* label
   B200_REQUIRE(!h->ops.empty(), "profile_ops: no plan bound");
   const long long n = (long long)(h->ops.size() + h->ops2.size());
   B200_REQUIRE(cap >= n, "profile_ops: need room for %lld ops", n);
-  set_call_args(h, x, labels, uniform, out);
-  h->in_v = x; h->tout = out;   // tangent plans: the JVP pass along v = x
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& e : ev) B200_CHECK_CUDA(cudaEventCreate(&e));
-  int rc = 0;
-  B200_CHECK_CUDA(cudaEventRecord(ev[0], st));
-  for (long long i = 0; i < n && !rc; ++i) {
-    rc = (i < (long long)h->ops.size() ? h->ops[i] : h->ops2[i - h->ops.size()]).fn(st);
-    cudaEventRecord(ev[i + 1], st);
-  }
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) { set_error("profile_ops: stream sync failed"); rc = 1; }
-  if (!rc) for (long long i = 0; i < n; ++i) cudaEventElapsedTime(&ms_per_op[i], ev[i], ev[i + 1]);
-  for (auto& e : ev) cudaEventDestroy(e);
-  return rc;
+  return time_ops(h, x, labels, uniform, out, stream, ms_per_op, "profile_ops");
 }
 
 int b200_ncsnpp_tap(b200_ncsnpp_t* h, int module_index, float* dst, long long cap, int shape_out[4], void* stream) {
@@ -1575,12 +1553,14 @@ long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h) { return h ? 
 // ===========================================================================
 // C ABI: predictor-corrector loop
 // ===========================================================================
+// per-step schedule tables of a PC plan (b200_pc_config: label .. cs); cm and cs only in constrained plans
+enum PcTable { PC_LABEL, PC_SS, PC_ALPHA, PC_PA, PC_PB, PC_PC, PC_CA, PC_CB, PC_CC, PC_CM, PC_CS, PC_TABLES };
+
 struct b200_pc {
   b200_ncsnpp* model; b200_pc_config cfg; int B; long long numel, per_img;
-  std::vector<float> h_label, h_ss, h_alpha, h_pa, h_pb, h_pc, h_ca, h_cb, h_cc, h_cm, h_cs;
+  std::vector<float> h_tab[PC_TABLES];   // host copies, uploaded by b200_pc_bind_workspace
   // workspace carve-up
-  char* ws = nullptr; float *d_label, *d_ss, *d_alpha, *d_pa, *d_pb, *d_pc, *d_ca, *d_cb, *d_cc, *labels, *net_out, *norms, *means;
-  float *d_cm = nullptr, *d_cs = nullptr;
+  char* ws = nullptr; float* d_tab[PC_TABLES] = {}; float *labels, *net_out, *norms, *means;
   int* d_step; unsigned long long* d_offset;
   PhiloxMap map;
   const float* known = nullptr; const float* mask = nullptr;   // constrained plans: bound by b200_pc_bind_constraint
@@ -1599,13 +1579,10 @@ long long pc_ws_layout(b200_pc* pc, char* base) {
   long long off = 0;
   auto take = [&](long long bytes) { long long o = off; off += (bytes + 255) & ~255LL; return base ? base + o : nullptr; };
   const int N = pc->cfg.n_steps;
-  pc->d_label = (float*)take(N * 4LL); pc->d_ss = (float*)take(N * 4LL); pc->d_alpha = (float*)take(N * 4LL);
-  pc->d_pa = (float*)take(N * 4LL); pc->d_pb = (float*)take(N * 4LL); pc->d_pc = (float*)take(N * 4LL);
-  pc->d_ca = (float*)take(N * 4LL); pc->d_cb = (float*)take(N * 4LL); pc->d_cc = (float*)take(N * 4LL);
+  for (int k = 0; k < PC_TABLES; ++k) if (k < PC_CM || pc->cfg.constraint) pc->d_tab[k] = (float*)take(N * 4LL);
   pc->labels = (float*)take(pc->B * 4LL); pc->net_out = (float*)take(pc->numel * 4LL);
   pc->norms = (float*)take(2LL * pc->B * 4); pc->means = (float*)take(256);
   pc->d_step = (int*)take(256); pc->d_offset = (unsigned long long*)take(256);
-  if (pc->cfg.constraint) { pc->d_cm = (float*)take(N * 4LL); pc->d_cs = (float*)take(N * 4LL); }
   return off;
 }
 
@@ -1616,8 +1593,8 @@ unsigned long long pc_calls_per_step(const b200_pc_config& c) {
 
 int pc_constrain(b200_pc* pc, float* x, float* x_mean, unsigned long long cps, unsigned long long call, cudaStream_t st) {
   const b200_ncsnpp_config& mc = pc->model->cfg;
-  return launch_pc_constrain(x, x_mean, pc->known, pc->mask, pc->map, pc->d_offset, pc->d_step, cps, call, pc->d_cm,
-                             pc->d_cs, pc->color, pc->cfg.constraint == 2, mc.num_channels,
+  return launch_pc_constrain(x, x_mean, pc->known, pc->mask, pc->map, pc->d_offset, pc->d_step, cps, call, pc->d_tab[PC_CM],
+                             pc->d_tab[PC_CS], pc->color, pc->cfg.constraint == 2, mc.num_channels,
                              (long long)mc.image_size * mc.image_size, st);
 }
 
@@ -1625,14 +1602,15 @@ int pc_constrain(b200_pc* pc, float* x, float* x_mean, unsigned long long cps, u
 int pc_iteration(b200_pc* pc, float* x, float* x_mean, const float* noise_c, const float* noise_p, cudaStream_t st) {
   b200_ncsnpp* m = pc->model;
   const b200_pc_config& c = pc->cfg;
-  PcStepScalars sc{pc->d_ss, pc->d_alpha, pc->d_pa, pc->d_pb, pc->d_pc};
+  float* const* t = pc->d_tab;
+  PcStepScalars sc{t[PC_SS], t[PC_ALPHA], t[PC_PA], t[PC_PB], t[PC_PC]};
   const unsigned long long cps = pc_calls_per_step(c);
-  if (int r = launch_fill_from_table(pc->d_label, pc->d_step, pc->labels, pc->B, st)) return r;
+  if (int r = launch_fill_from_table(t[PC_LABEL], pc->d_step, pc->labels, pc->B, st)) return r;
   unsigned long long call = 0;
   if (c.corrector == 2) {
     // affine corrector (annealed Langevin dynamics, sampling.py:286-319): the step size is a per-step scalar, so the update is
     // the predictor's kernel with the corrector's own tables; every inner step draws fresh noise like the reference's loop
-    PcStepScalars cs{pc->d_ss, pc->d_alpha, pc->d_ca, pc->d_cb, pc->d_cc};
+    PcStepScalars cs{t[PC_SS], t[PC_ALPHA], t[PC_CA], t[PC_CB], t[PC_CC]};
     for (int k = 0; k < c.n_corrector_steps; ++k) {
       if (int r = b200_ncsnpp_forward(m, x, pc->labels, 1, pc->net_out, st)) return r;
       if (int r = launch_predictor_apply(x, x_mean, pc->net_out, noise_c, pc->map, pc->d_offset, pc->d_step, cps, call, cs, 1, st)) return r;
@@ -1692,18 +1670,21 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   pc->per_img = (long long)mc.num_channels * mc.image_size * mc.image_size;
   pc->numel = pc->per_img * batch;
   const int N = cfg->n_steps;
-  auto cp = [&](std::vector<float>& dst, const float* src, float dflt) { dst.assign(N, dflt); if (src) memcpy(dst.data(), src, N * 4); };
-  cp(pc->h_label, cfg->label, 0.f); cp(pc->h_ss, cfg->score_scale, 1.f); cp(pc->h_alpha, cfg->alpha, 1.f);
-  cp(pc->h_pa, cfg->pa, 1.f); cp(pc->h_pb, cfg->pb, 0.f); cp(pc->h_pc, cfg->pc, 0.f);
-  cp(pc->h_ca, cfg->ca, 1.f); cp(pc->h_cb, cfg->cb, 0.f); cp(pc->h_cc, cfg->cc, 0.f);
-  pc->cfg.label = pc->cfg.score_scale = pc->cfg.alpha = pc->cfg.pa = pc->cfg.pb = pc->cfg.pc = nullptr;
-  pc->cfg.ca = pc->cfg.cb = pc->cfg.cc = nullptr;
+  // a table the caller leaves null takes its default: label 0, score_scale 1, alpha 1, the predictor's and the
+  // corrector's x_mean = 1 x + 0 out, x = x_mean + 0 z, and the constraint's marginal 1 known + 0 z
+  const float* src[PC_TABLES] = {cfg->label, cfg->score_scale, cfg->alpha, cfg->pa, cfg->pb, cfg->pc, cfg->ca, cfg->cb, cfg->cc, cfg->cm, cfg->cs};
+  const float dflt[PC_TABLES] = {0.f, 1.f, 1.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f, 1.f, 0.f};
+  for (int k = 0; k < PC_TABLES; ++k) {
+    if (k >= PC_CM && !cfg->constraint) continue;
+    pc->h_tab[k].assign(N, dflt[k]);
+    if (src[k]) memcpy(pc->h_tab[k].data(), src[k], N * 4);
+  }
   if (cfg->constraint) {
-    cp(pc->h_cm, cfg->cm, 1.f); cp(pc->h_cs, cfg->cs, 0.f);
     memcpy(pc->color.M, cfg->color_m, sizeof(pc->color.M));
     memcpy(pc->color.Minv, cfg->color_minv, sizeof(pc->color.Minv));
   }
-  pc->cfg.cm = pc->cfg.cs = nullptr;
+  pc->cfg.label = pc->cfg.score_scale = pc->cfg.alpha = pc->cfg.pa = pc->cfg.pb = pc->cfg.pc = nullptr;
+  pc->cfg.ca = pc->cfg.cb = pc->cfg.cc = pc->cfg.cm = pc->cfg.cs = nullptr;
   const long long cps = (cfg->corrector ? cfg->n_corrector_steps : 0) + (cfg->predictor ? 1 : 0);   // network evaluations
   const long long tail = cfg->constraint ? (cfg->predictor ? 1 : 0) + 2   /* predictor apply, two blends */
                                          : 1 /* predictor apply, or the x -> x_mean copy */;
@@ -1729,19 +1710,8 @@ int b200_pc_bind_workspace(b200_pc_t* pc, void* ws, long long bytes, void* strea
   pc->ws = base;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int N = pc->cfg.n_steps;
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_label, pc->h_label.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_ss, pc->h_ss.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_alpha, pc->h_alpha.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_pa, pc->h_pa.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_pb, pc->h_pb.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_pc, pc->h_pc.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_ca, pc->h_ca.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cb, pc->h_cb.data(), N * 4, cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cc, pc->h_cc.data(), N * 4, cudaMemcpyHostToDevice, st));
-  if (pc->cfg.constraint) {
-    B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cm, pc->h_cm.data(), N * 4, cudaMemcpyHostToDevice, st));
-    B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_cs, pc->h_cs.data(), N * 4, cudaMemcpyHostToDevice, st));
-  }
+  for (int k = 0; k < PC_TABLES; ++k)
+    if (pc->d_tab[k]) B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_tab[k], pc->h_tab[k].data(), N * 4, cudaMemcpyHostToDevice, st));
   B200_CHECK_CUDA(cudaStreamSynchronize(st));
   if (pc->gexec) { cudaGraphExecDestroy(pc->gexec); pc->gexec = nullptr; }
   if (int r = philox_map_init(&pc->map, pc->numel, 0)) return r;
