@@ -262,12 +262,13 @@ B200_API int b200_pc_step_external(b200_pc_t* pc, float* x, float* x_mean, int s
                                    const float* noise_corrector, const float* noise_predictor, void* stream);
 B200_API long long b200_pc_launches_per_step(const b200_pc_t* pc);
 
-/* ---- probability-flow ODE sampler: device-resident Dormand-Prince 5(4) -------------------------
- * Replaces the host-side state and stage arithmetic of sampling.py:414-485 (scipy.integrate.solve_ivp on a float64
- * numpy array: two PCIe crossings of the whole state per function evaluation).  The float64 state y, y_new and the
- * seven stage derivatives K[7][n] stay in device memory; scipy's step-size controller runs on the host
- * (score_sde_pytorch_b200/ode.py) and reads back one double per attempted step.  All pointers are device pointers
- * except coef_host / e_host (<= 8 doubles, passed by value into the launch). */
+/* ---- probability-flow ODE: device-resident explicit Runge-Kutta (RK23, RK45, DOP853) ------------
+ * Replaces the host-side state and stage arithmetic of sampling.py:414-485 and likelihood.py:84-113
+ * (scipy.integrate.solve_ivp on a float64 numpy array: two PCIe crossings of the whole state per function evaluation).
+ * The float64 state y, y_new and the stage derivatives K[n_stages + 1][n] stay in device memory; scipy's step-size
+ * controller runs on the host (score_sde_pytorch_b200/ode.py) and reads back one double per attempted step (two for
+ * DOP853).  All pointers are device pointers except coef_host / e_host / e5_host / e3_host (<= 16 doubles, passed by
+ * value into the launch). */
 /* y_stage = y + h * sum_{j<nk} coef[j] * K[j] (float64; nk = 0: y itself); optional float64 copy (y_out) and float32
  * copy (x32: the network input, `.type(torch.float32)` in the reference's ode_func) */
 B200_API int b200_ode_stage_f64(const double* y, const double* k, long long n, const double* coef_host, int nk, double h,
@@ -287,6 +288,12 @@ B200_API int b200_ode_div_f64(const float* eps, const float* jvp_out, int nimg, 
 B200_API long long b200_ode_workspace_doubles(void);
 B200_API int b200_ode_error_sumsq_f64(const double* y, const double* y_new, const double* k, long long n, const double* e_host,
                                       int nk, double h, double rtol, double atol, double* ws, void* stream);
+/* DOP853._estimate_error_norm's two sums from one read of K, scale_i = atol + max(|y_i|, |y_new_i|) * rtol:
+ * ws[0] = sum_i ((sum_{j<nk} e5[j] K[j][i]) / scale_i)^2,  ws[1] = sum_i ((sum_{j<nk} e3[j] K[j][i]) / scale_i)^2;
+ * each the same deterministic two-pass reduction as b200_ode_error_sumsq_f64 */
+B200_API int b200_ode_error_sumsq2_f64(const double* y, const double* y_new, const double* k, long long n,
+                                       const double* e5_host, const double* e3_host, int nk, double rtol, double atol,
+                                       double* ws, void* stream);
 /* ws[0] = sum_i (((v - v2)_i) / (atol + |y0_i| * rtol))^2, v2 optional: the three norms of scipy's select_initial_step */
 B200_API int b200_ode_scaled_sumsq_f64(const double* v, const double* v2, const double* y0, long long n, double rtol, double atol,
                                        double* ws, void* stream);

@@ -101,6 +101,8 @@ SIGNATURES = {
   'b200_ode_workspace_doubles': (c_ll, []),
   'b200_ode_error_sumsq_f64': (c_int, [c_void_p, c_void_p, c_void_p, c_ll, P(ctypes.c_double), c_int, ctypes.c_double,
                                        ctypes.c_double, ctypes.c_double, c_void_p, c_void_p]),
+  'b200_ode_error_sumsq2_f64': (c_int, [c_void_p, c_void_p, c_void_p, c_ll, P(ctypes.c_double), P(ctypes.c_double), c_int,
+                                        ctypes.c_double, ctypes.c_double, c_void_p, c_void_p]),
   'b200_ode_scaled_sumsq_f64': (c_int, [c_void_p, c_void_p, c_void_p, c_ll, ctypes.c_double, ctypes.c_double, c_void_p, c_void_p]),
   'b200_dsm_perturb_f32': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_ll, c_void_p]),
   'b200_dsm_workspace_doubles': (c_ll, [c_int, c_ll]),

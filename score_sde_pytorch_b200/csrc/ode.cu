@@ -1,11 +1,12 @@
-// Device-resident pieces of the probability-flow ODE sampler (sampling.py:414-485 in the reference).
+// Device-resident pieces of the probability-flow ODE solver (sampling.py:414-485 and likelihood.py:84-113 in the reference).
 //
-// The reference integrates dx/dt = f(x,t) - 1/2 g(t)^2 score(x,t) with scipy.integrate.solve_ivp(method='RK45'): the state
+// The reference integrates dx/dt = f(x,t) - 1/2 g(t)^2 score(x,t) with scipy.integrate.solve_ivp(method=m): the state
 // lives in a float64 numpy array on the HOST, every right-hand side copies it to the GPU (as float32), evaluates the
 // network, and copies the drift back - two PCIe crossings of the whole state per function evaluation, plus numpy's
-// stage arithmetic on one host core.  Here the float64 state, the seven Dormand-Prince stage derivatives and all
-// stage / error arithmetic stay in HBM; the host keeps scipy's step-size controller (a handful of float64 scalars,
-// score_sde_pytorch_b200/ode.py) and reads back ONE double per attempted step: the sum of squares behind the error norm.
+// stage arithmetic on one host core.  Here the float64 state, the Runge-Kutta stage derivatives (RK23: 4, RK45: 7,
+// DOP853: 13) and all stage / error arithmetic stay in HBM; the host keeps scipy's step-size controller (a handful of
+// float64 scalars, score_sde_pytorch_b200/ode.py) and reads back the sum of squares behind the error norm once per
+// attempted step (one double; two for DOP853's two error estimators).
 //
 // Arithmetic follows the reference's: stage states and y_new in float64 (numpy), the network input and the drift in
 // float32 with torch's operation order (sde_lib.py:93-100: drift - diffusion^2 * score * 0.5, unfused), the drift widened
@@ -19,7 +20,10 @@ namespace {
 constexpr int ODE_THREADS = 256;
 constexpr int ODE_MAX_BLOCKS = 1024;
 
-struct OdeCoef { double c[8]; };
+// DOP853: 12 stage weights, 13 error weights.  The coefficient loops run unrolled to this bound (guarded by nk) so the
+// coefficients are read from the kernel parameters at fixed offsets, not from a per-thread local copy.
+constexpr int ODE_MAX_COEF = 16;
+struct OdeCoef { double c[ODE_MAX_COEF]; };
 
 // y_stage = y + h * sum_j c[j] K[j];  optional float64 copy (y_new), float32 copy (network input)
 __global__ void __launch_bounds__(ODE_THREADS) ode_stage_kernel(const double* __restrict__ y, const double* __restrict__ K,
@@ -28,7 +32,9 @@ __global__ void __launch_bounds__(ODE_THREADS) ode_stage_kernel(const double* __
   pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     double acc = 0.0;
-    for (int j = 0; j < nk; ++j) acc += K[(long long)j * n + i] * coef.c[j];       // np.dot(K[:s].T, a[:s])
+#pragma unroll
+    for (int j = 0; j < ODE_MAX_COEF; ++j)                                         // np.dot(K[:s].T, a[:s])
+      if (j < nk) acc += K[(long long)j * n + i] * coef.c[j];
     const double v = nk ? y[i] + acc * h : y[i];                                   // y + dy, dy = dot * h
     if (y_out) y_out[i] = v;
     if (x32) x32[i] = (float)v;                                                    // .type(torch.float32)
@@ -83,6 +89,22 @@ __device__ __forceinline__ void block_sum_to(double v, double* dst) {
   }
 }
 
+// block_sum_to for two values at once (one barrier): each sum in block_sum_to's order
+__device__ __forceinline__ void block_sum2_to(double a, double b, double* dst_a, double* dst_b) {
+  __shared__ double sh[2][ODE_THREADS / 32];
+  a = warp_sum_d(a);
+  b = warp_sum_d(b);
+  if ((threadIdx.x & 31) == 0) { sh[0][threadIdx.x >> 5] = a; sh[1][threadIdx.x >> 5] = b; }
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    double ta = threadIdx.x < ODE_THREADS / 32 ? sh[0][threadIdx.x] : 0.0;
+    double tb = threadIdx.x < ODE_THREADS / 32 ? sh[1][threadIdx.x] : 0.0;
+    ta = warp_sum_d(ta);
+    tb = warp_sum_d(tb);
+    if (threadIdx.x == 0) { *dst_a = ta; *dst_b = tb; }
+  }
+}
+
 // partial[b] = sum over this block's elements of ((h * sum_j e[j] K[j][i]) / (atol + max(|y|, |y_new|) * rtol))^2
 __global__ void __launch_bounds__(ODE_THREADS) ode_error_kernel(const double* __restrict__ y, const double* __restrict__ y_new,
                                                                 const double* __restrict__ K, long long n, OdeCoef e, int nk,
@@ -91,12 +113,40 @@ __global__ void __launch_bounds__(ODE_THREADS) ode_error_kernel(const double* __
   double s = 0.0;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     double acc = 0.0;
-    for (int j = 0; j < nk; ++j) acc += K[(long long)j * n + i] * e.c[j];
+#pragma unroll
+    for (int j = 0; j < ODE_MAX_COEF; ++j)
+      if (j < nk) acc += K[(long long)j * n + i] * e.c[j];
     const double scale = atol + fmax(fabs(y[i]), fabs(y_new[i])) * rtol;
     const double r = acc * h / scale;
     s += r * r;
   }
   block_sum_to(s, partial + blockIdx.x);
+}
+
+// DOP853's two estimators from one read of K: partial5[b] / partial3[b] = sum over this block's elements of
+// ((sum_j e5[j] K[j][i]) / scale)^2 / ((sum_j e3[j] K[j][i]) / scale)^2, scale = atol + max(|y|, |y_new|) * rtol
+__global__ void __launch_bounds__(ODE_THREADS) ode_error2_kernel(const double* __restrict__ y, const double* __restrict__ y_new,
+                                                                 const double* __restrict__ K, long long n, OdeCoef e5,
+                                                                 OdeCoef e3, int nk, double rtol, double atol,
+                                                                 double* __restrict__ partial5, double* __restrict__ partial3) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  double s5 = 0.0, s3 = 0.0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    double acc5 = 0.0, acc3 = 0.0;
+#pragma unroll
+    for (int j = 0; j < ODE_MAX_COEF; ++j) {
+      if (j < nk) {
+        const double k = K[(long long)j * n + i];
+        acc5 += k * e5.c[j];
+        acc3 += k * e3.c[j];
+      }
+    }
+    const double scale = atol + fmax(fabs(y[i]), fabs(y_new[i])) * rtol;
+    const double r5 = acc5 / scale, r3 = acc3 / scale;
+    s5 += r5 * r5;
+    s3 += r3 * r3;
+  }
+  block_sum2_to(s5, s3, partial5 + blockIdx.x, partial3 + blockIdx.x);
 }
 
 // partial[b] = sum of ((v - v2) / (atol + |y0| * rtol))^2     (v2 optional) : the norms of select_initial_step
@@ -131,8 +181,8 @@ extern "C" {
 
 int b200_ode_stage_f64(const double* y, const double* k, long long n, const double* coef_host, int nk, double h,
                        double* y_out, float* x32, void* stream) {
-  B200_REQUIRE(y && n > 0 && nk >= 0 && nk <= 8 && (nk == 0 || (k && coef_host)), "ode_stage: bad argument");
-  OdeCoef c; for (int j = 0; j < 8; ++j) c.c[j] = j < nk ? coef_host[j] : 0.0;
+  B200_REQUIRE(y && n > 0 && nk >= 0 && nk <= ODE_MAX_COEF && (nk == 0 || (k && coef_host)), "ode_stage: bad argument");
+  OdeCoef c; for (int j = 0; j < ODE_MAX_COEF; ++j) c.c[j] = j < nk ? coef_host[j] : 0.0;
   launch_kernel(ode_stage_kernel, dim3(ode_grid(n)), dim3(ODE_THREADS), 0, static_cast<cudaStream_t>(stream), y, k, n, c, nk, h, y_out, x32);
   B200_CHECK_LAUNCH();
   return 0;
@@ -154,16 +204,33 @@ int b200_ode_div_f64(const float* eps, const float* jvp_out, int nimg, long long
   return 0;
 }
 
-long long b200_ode_workspace_doubles(void) { return ODE_MAX_BLOCKS + 8; }
+// ws[0..7]: results; ws + 8: block partials (two arrays of ODE_MAX_BLOCKS for b200_ode_error_sumsq2_f64)
+long long b200_ode_workspace_doubles(void) { return 2 * ODE_MAX_BLOCKS + 8; }
 
 int b200_ode_error_sumsq_f64(const double* y, const double* y_new, const double* k, long long n, const double* e_host, int nk,
                              double h, double rtol, double atol, double* ws, void* stream) {
-  B200_REQUIRE(y && y_new && k && e_host && ws && n > 0 && nk > 0 && nk <= 8, "ode_error: bad argument");
-  OdeCoef c; for (int j = 0; j < 8; ++j) c.c[j] = j < nk ? e_host[j] : 0.0;
+  B200_REQUIRE(y && y_new && k && e_host && ws && n > 0 && nk > 0 && nk <= ODE_MAX_COEF, "ode_error: bad argument");
+  OdeCoef c; for (int j = 0; j < ODE_MAX_COEF; ++j) c.c[j] = j < nk ? e_host[j] : 0.0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int g = ode_grid(n);
   launch_kernel(ode_error_kernel, dim3(g), dim3(ODE_THREADS), 0, st, y, y_new, k, n, c, nk, h, rtol, atol, ws + 8);
   launch_kernel(ode_final_sum_kernel, dim3(1), dim3(ODE_THREADS), 0, st, ws + 8, g, ws);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+int b200_ode_error_sumsq2_f64(const double* y, const double* y_new, const double* k, long long n, const double* e5_host,
+                              const double* e3_host, int nk, double rtol, double atol, double* ws, void* stream) {
+  B200_REQUIRE(y && y_new && k && e5_host && e3_host && ws && n > 0 && nk > 0 && nk <= ODE_MAX_COEF, "ode_error2: bad argument");
+  OdeCoef c5, c3;
+  for (int j = 0; j < ODE_MAX_COEF; ++j) { c5.c[j] = j < nk ? e5_host[j] : 0.0; c3.c[j] = j < nk ? e3_host[j] : 0.0; }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int g = ode_grid(n);
+  double* p5 = ws + 8;
+  double* p3 = ws + 8 + ODE_MAX_BLOCKS;
+  launch_kernel(ode_error2_kernel, dim3(g), dim3(ODE_THREADS), 0, st, y, y_new, k, n, c5, c3, nk, rtol, atol, p5, p3);
+  launch_kernel(ode_final_sum_kernel, dim3(1), dim3(ODE_THREADS), 0, st, p5, g, ws);
+  launch_kernel(ode_final_sum_kernel, dim3(1), dim3(ODE_THREADS), 0, st, p3, g, ws + 1);
   B200_CHECK_LAUNCH();
   return 0;
 }

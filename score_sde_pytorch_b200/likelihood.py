@@ -6,10 +6,11 @@ The reference's Hutchinson-Skilling estimator is ``eps . (J_drift^T eps)``, a ve
 engine-backed networks provide that one as a forward-mode tangent pass (``EngineModel.jvp``, ``b200_ncsnpp_jvp``): no
 backward graph, no stored activations.
 
-With an engine-backed network whose configuration the tangent pass supports, ``method='RK45'``, a stock VE / VP / sub-VP
-SDE and CUDA data, the probability-flow ODE over the augmented state ``[x; logp]`` is integrated device-resident
-(``ode.py`` + ``csrc/ode.cu``): float64 state and Dormand-Prince stages in HBM, scipy's step-size controller on the host,
-one primal+tangent network evaluation per right-hand side.  Other ``method`` values, user SDEs, CPU data and
+With an engine-backed network whose configuration the tangent pass supports, an explicit Runge-Kutta ``method``
+(``'RK23'``, ``'RK45'`` or ``'DOP853'``), a stock VE / VP / sub-VP SDE and CUDA data, the probability-flow ODE over the
+augmented state ``[x; logp]`` is integrated device-resident (``ode.py`` + ``csrc/ode.cu``): float64 state and Runge-Kutta
+stages in HBM, scipy's step-size controller on the host, one primal+tangent network evaluation per right-hand side.  The
+implicit methods ``'Radau'``, ``'BDF'`` and ``'LSODA'`` (they need the Jacobian), user SDEs, CPU data and
 ``device_solver=False`` run the reference's loop over ``scipy.integrate.solve_ivp``; its divergence comes from autograd
 for a plain ``nn.Module`` (as in the reference) and from ``model.jvp`` for an engine-backed network, whose forward has no
 autograd graph.  An engine-backed network whose configuration has no tangent pass raises ``NotImplementedError``.
@@ -70,7 +71,8 @@ def get_likelihood_fn(sde, inverse_scaler, hutchinson_type='Rademacher',
   """Create a function to compute the unbiased log-likelihood estimate of a given data point (``likelihood.py:40-113``).
 
   ``device_solver``: ``None`` picks the device-resident solve when it applies, ``False`` forces the host loop, ``True``
-  requires the device solve (``NotImplementedError`` otherwise).  ``likelihood_fn.last_stats`` records which ran."""
+  requires the device solve (``NotImplementedError`` otherwise).  ``likelihood_fn.last_stats`` records which solver ran
+  and the method."""
 
   def drift_fn(model, x, t):
     """The drift function of the reverse-time SDE."""
@@ -83,12 +85,17 @@ def get_likelihood_fn(sde, inverse_scaler, hutchinson_type='Rademacher',
     return get_div_fn(lambda xx, tt: drift_fn(model, xx, tt))(x, t, noise)
 
   def use_device_solver(net, data):
-    ok = net is not None and method == 'RK45' and data.is_cuda and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
+    from . import ode as _ode
     if device_solver is False:
       return False
+    if device_solver and method not in _ode.METHODS:
+      raise NotImplementedError(f'get_likelihood_fn(device_solver=True): method {method!r} has no device solve '
+                                f'(explicit Runge-Kutta methods only: {", ".join(_ode.METHODS)})')
+    ok = (net is not None and method in _ode.METHODS and data.is_cuda
+          and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE))
     if device_solver and not ok:
       raise NotImplementedError('get_likelihood_fn(device_solver=True) needs an engine-backed network (NCSNpp or DDPM), '
-                                "method='RK45', a VE/VP/sub-VP SDE and CUDA data")
+                                "a VE/VP/sub-VP SDE and CUDA data")
     return ok
 
   def likelihood_fn(model, data, epsilon=None):
@@ -118,12 +125,13 @@ def get_likelihood_fn(sde, inverse_scaler, hutchinson_type='Rademacher',
         net.check_jvp_supported()             # NotImplementedError before any launch: there is nothing to fall back to
       if use_device_solver(net, data):
         from . import ode as _ode
+        solver = _ode.METHODS[method]
         ops = _ode.CudaOdeOps(data.to(torch.float32), _ode.engine_likelihood_fn(sde, net, epsilon.to(torch.float32)),
-                              extra=shape[0])
-        nfe = _ode.DormandPrince45(ops, eps, sde.T, rtol=rtol, atol=atol).solve()
+                              extra=shape[0], method=solver)
+        nfe = solver(ops, eps, sde.T, rtol=rtol, atol=atol).solve()
         z = ops.state_f32()
         delta_logp = ops.extra_state().to(torch.float32)
-        likelihood_fn.last_stats = dict(nfev=nfe, host_scalar_reads=ops.host_reads, solver='device')
+        likelihood_fn.last_stats = dict(nfev=nfe, host_scalar_reads=ops.host_reads, solver='device', method=method)
       else:
         def ode_func(t, x):
           sample = mutils.from_flattened_numpy(x[:-shape[0]], shape).to(data.device).type(torch.float32)
@@ -142,7 +150,7 @@ def get_likelihood_fn(sde, inverse_scaler, hutchinson_type='Rademacher',
         zp = solution.y[:, -1]
         z = mutils.from_flattened_numpy(zp[:-shape[0]], shape).to(data.device).type(torch.float32)
         delta_logp = mutils.from_flattened_numpy(zp[-shape[0]:], (shape[0],)).to(data.device).type(torch.float32)
-        likelihood_fn.last_stats = dict(nfev=nfe, solver='scipy')
+        likelihood_fn.last_stats = dict(nfev=nfe, solver='scipy', method=method)
       prior_logp = sde.prior_logp(z)
       bpd = -(prior_logp + delta_logp) / np.log(2)
       N = np.prod(shape[1:])

@@ -1,52 +1,64 @@
-"""Device-resident probability-flow ODE sampler (successor of ``sampling.py:414-485``'s host-side scipy loop).
+"""Device-resident probability-flow ODE solver (successor of the host-side scipy loops of ``sampling.py:414-485`` and
+``likelihood.py:84-113``).
 
-``scipy.integrate.solve_ivp(method='RK45')`` keeps the state in a float64 numpy array and calls the right-hand side
-with it: in the reference every function evaluation moves the whole batch host -> device -> host.  Here the float64
-state, the seven Dormand-Prince stage derivatives and every stage / error sum live in HBM (``csrc/ode.cu`` behind
-``b200_ode_*``); this module is scipy's step-size CONTROLLER restated on Python floats (IEEE doubles, like numpy's):
-``select_initial_step`` (``scipy/integrate/_ivp/common.py``), ``RungeKutta._step_impl`` and ``rk_step``
-(``_ivp/rk.py``), and ``solve_ivp``'s outer loop without events / dense output.  One double per attempted step
-crosses PCIe (the sum of squares behind the error norm); the accepted/rejected decision is taken on the host exactly as
-scipy takes it, so the trajectory of step sizes - and ``nfev`` - follow scipy's for the same right-hand side.
+``scipy.integrate.solve_ivp(method=m)`` keeps the state in a float64 numpy array and calls the right-hand side with it:
+in the reference every function evaluation moves the whole batch host -> device -> host.  Here the float64 state, the
+Runge-Kutta stage derivatives and every stage / error sum live in HBM (``csrc/ode.cu`` behind ``b200_ode_*``); this
+module is scipy's step-size CONTROLLER restated on Python floats (IEEE doubles, like numpy's): ``select_initial_step``
+(``scipy/integrate/_ivp/common.py``), ``RungeKutta._step_impl``, ``_estimate_error_norm`` and ``rk_step``
+(``_ivp/rk.py``), and ``solve_ivp``'s outer loop without events / dense output.  It covers scipy's three explicit
+Runge-Kutta pairs, with scipy's own coefficient arrays:
 
-:class:`DormandPrince45` is arithmetic-agnostic: it drives an ``ops`` object (``CudaOdeOps`` below; the CPU tests
-plug a numpy one in to compare the controller with scipy itself).
+  ``RK23``    Bogacki-Shampine 3(2): 3 stages + FSAL, error estimator order 2
+  ``RK45``    Dormand-Prince 5(4): 6 stages + FSAL, error estimator order 4 (:class:`DormandPrince45`)
+  ``DOP853``  Dormand-Prince 8(5,3): 12 stages + FSAL, error estimator order 7, scipy's combined 5th/3rd-order error norm
+
+One transfer per attempted step crosses PCIe (the sum of squares behind the error norm; for DOP853 the two sums of its
+two estimators); the accepted/rejected decision is taken on the host exactly as scipy takes it, so the trajectory of step
+sizes - and ``nfev`` - follow scipy's for the same right-hand side.  ``Radau``, ``BDF`` and ``LSODA`` are implicit
+methods that need the Jacobian of the right-hand side; they have no device solve.
+
+:class:`RungeKutta` is arithmetic-agnostic: it drives an ``ops`` object (``CudaOdeOps`` below; the CPU tests plug a
+numpy one in to compare the controller with scipy itself).
 """
 import ctypes
 import math
 
 import torch
+from scipy import integrate as _scipy
 
 from . import _lib
 
-# Dormand-Prince 5(4) tableau (scipy/integrate/_ivp/rk.py: class RK45)
-C = (0.0, 1 / 5, 3 / 10, 4 / 5, 8 / 9, 1.0)
-A = ((),
-     (1 / 5,),
-     (3 / 40, 9 / 40),
-     (44 / 45, -56 / 15, 32 / 9),
-     (19372 / 6561, -25360 / 2187, 64448 / 6561, -212 / 729),
-     (9017 / 3168, -355 / 33, 46732 / 5247, 49 / 176, -5103 / 18656))
-B = (35 / 384, 0.0, 500 / 1113, 125 / 192, -2187 / 6784, 11 / 84)
-E = (-71 / 57600, 0.0, 71 / 16695, -71 / 1920, 17253 / 339200, -22 / 525, 1 / 40)
-ORDER, ERROR_ESTIMATOR_ORDER, N_STAGES = 5, 4, 6
+
+def _tableau(cls):
+  """(C, A, B) of a scipy ``RungeKutta`` class as Python floats; row s of A holds the s coefficients ``rk_step`` uses."""
+  return (tuple(float(c) for c in cls.C), tuple(tuple(float(a) for a in cls.A[s, :s]) for s in range(cls.n_stages)),
+          tuple(float(b) for b in cls.B))
+
+
 SAFETY, MIN_FACTOR, MAX_FACTOR = 0.9, 0.2, 10.0     # _ivp/rk.py module constants
 
 
-class DormandPrince45:
-  """``ops`` provides (all state stays wherever ``ops`` keeps it; K[j] is stage-derivative slot j of 7):
+class RungeKutta:
+  """``ops`` provides (all state stays wherever ``ops`` keeps it; K[j] is stage-derivative slot j of n_stages + 1):
       ops.n                                  number of state elements
       ops.rhs(t, coefs, h, slot, keep_y)     K[slot] = f(t, y + h * sum_j coefs[j] K[j]); keep_y: also store that state as y_new
       ops.error_sumsq(h, rtol, atol)         sum(((h * sum_j E[j] K[j]) / (atol + max(|y|, |y_new|) * rtol))**2)
+      ops.error_sumsq2(rtol, atol)           DOP853 only: the same sum without h for E5 and for E3, as a pair
       ops.scaled_sumsq(slot, minus, rtol, atol)   sum(((K[slot] - K[minus]) / (atol + |y| * rtol))**2), slot=-1: y itself
-      ops.accept()                           y <- y_new, K[0] <- K[6]
-  """
+      ops.accept()                           y <- y_new, K[0] <- K[n_stages]
+
+  The norm divides by ``math.sqrt(n)``; scipy's ``x.size ** 0.5`` goes through libm's ``pow``, which for about 0.1 % of
+  sizes rounds differently in the last bit."""
+  name = None
+  C = A = B = E = None
+  order = error_estimator_order = n_stages = None
 
   def __init__(self, ops, t0, t_bound, rtol=1e-5, atol=1e-5, max_step=math.inf):
     self.ops, self.t, self.t_bound = ops, float(t0), float(t_bound)
     self.rtol, self.atol, self.max_step = float(rtol), float(atol), max_step
     self.direction = (1.0 if t_bound > t0 else -1.0) if t_bound != t0 else 1.0
-    self.error_exponent = -1 / (ERROR_ESTIMATOR_ORDER + 1)
+    self.error_exponent = -1 / (self.error_estimator_order + 1)
     self.nfev = 0
     self.n_accepted = self.n_rejected = 0
     self._rhs(self.t, (), 0.0, 0, False)                      # self.f = self.fun(self.t, self.y)
@@ -58,6 +70,10 @@ class DormandPrince45:
 
   def _norm(self, sumsq):
     return math.sqrt(sumsq) / math.sqrt(self.ops.n)           # np.linalg.norm(x) / x.size ** 0.5
+
+  def _error_norm(self, h):
+    """RungeKutta._estimate_error_norm(K, h, scale)."""
+    return self._norm(self.ops.error_sumsq(h, self.rtol, self.atol))
 
   def _select_initial_step(self):
     """scipy/integrate/_ivp/common.py:select_initial_step (order = error_estimator_order)."""
@@ -73,7 +89,7 @@ class DormandPrince45:
     if d1 <= 1e-15 and d2 <= 1e-15:
       h1 = max(1e-6, h0 * 1e-3)
     else:
-      h1 = (0.01 / max(d1, d2)) ** (1 / (ERROR_ESTIMATOR_ORDER + 1))
+      h1 = (0.01 / max(d1, d2)) ** (1 / (self.error_estimator_order + 1))
     return min(100 * h0, h1, interval_length, self.max_step)
 
   def _step(self):
@@ -96,10 +112,10 @@ class DormandPrince45:
         t_new = self.t_bound
       h = t_new - t
       h_abs = abs(h)
-      for s in range(1, N_STAGES):                             # rk_step: K[s] = fun(t + c*h, y + (K[:s].T @ a[:s]) * h)
-        self._rhs(t + C[s] * h, A[s], h, s, False)
-      self._rhs(t + h, B, h, N_STAGES, True)                   # y_new = y + h * K[:-1].T @ B; K[-1] = fun(t + h, y_new)
-      error_norm = self._norm(self.ops.error_sumsq(h, self.rtol, self.atol))
+      for s in range(1, self.n_stages):                        # rk_step: K[s] = fun(t + c*h, y + (K[:s].T @ a[:s]) * h)
+        self._rhs(t + self.C[s] * h, self.A[s], h, s, False)
+      self._rhs(t + h, self.B, h, self.n_stages, True)         # y_new = y + h * K[:-1].T @ B; K[-1] = fun(t + h, y_new)
+      error_norm = self._error_norm(h)
       if error_norm < 1:
         factor = MAX_FACTOR if error_norm == 0 else min(MAX_FACTOR, SAFETY * error_norm ** self.error_exponent)
         if step_rejected:
@@ -120,18 +136,66 @@ class DormandPrince45:
     """solve_ivp's loop (no events, no dense output): step until t_bound.  Returns nfev."""
     while self.direction * (self.t - self.t_bound) < 0:
       if not self._step():
-        raise RuntimeError('RK45: required step size is less than spacing between numbers')   # solve_ivp status -1
+        raise RuntimeError(f'{self.name}: required step size is less than spacing between numbers')   # solve_ivp status -1
     return self.nfev
 
 
+class RK23(RungeKutta):
+  """scipy.integrate.RK23: Bogacki-Shampine 3(2)."""
+  name = 'RK23'
+  order, error_estimator_order, n_stages = _scipy.RK23.order, _scipy.RK23.error_estimator_order, _scipy.RK23.n_stages
+  C, A, B = _tableau(_scipy.RK23)
+  E = tuple(float(e) for e in _scipy.RK23.E)
+
+
+class DormandPrince45(RungeKutta):
+  """scipy.integrate.RK45: Dormand-Prince 5(4)."""
+  name = 'RK45'
+  order, error_estimator_order, n_stages = _scipy.RK45.order, _scipy.RK45.error_estimator_order, _scipy.RK45.n_stages
+  C, A, B = _tableau(_scipy.RK45)
+  E = tuple(float(e) for e in _scipy.RK45.E)
+
+
+class DOP853(RungeKutta):
+  """scipy.integrate.DOP853: Dormand-Prince 8(5,3), whose error norm combines a 5th- and a 3rd-order estimator."""
+  name = 'DOP853'
+  order, error_estimator_order, n_stages = _scipy.DOP853.order, _scipy.DOP853.error_estimator_order, _scipy.DOP853.n_stages
+  C, A, B = _tableau(_scipy.DOP853)
+  E5 = tuple(float(e) for e in _scipy.DOP853.E5)
+  E3 = tuple(float(e) for e in _scipy.DOP853.E3)
+
+  def _error_norm(self, h):
+    """DOP853._estimate_error_norm: |h| ||err5||^2 / sqrt((||err5||^2 + 0.01 ||err3||^2) n), err = K.E / scale."""
+    s5, s3 = self.ops.error_sumsq2(self.rtol, self.atol)
+    err5_norm_2, err3_norm_2 = math.sqrt(s5) ** 2, math.sqrt(s3) ** 2       # np.linalg.norm(err) ** 2
+    if err5_norm_2 == 0 and err3_norm_2 == 0:
+      return 0.0
+    denom = err5_norm_2 + 0.01 * err3_norm_2
+    return abs(h) * err5_norm_2 / math.sqrt(denom * self.ops.n)
+
+
+# the explicit methods of solve_ivp, by the name it takes
+METHODS = {'RK23': RK23, 'RK45': DormandPrince45, 'DOP853': DOP853}
+
+# Dormand-Prince 5(4) tableau under its earlier module-level names
+C, A, B, E = DormandPrince45.C, DormandPrince45.A, DormandPrince45.B, DormandPrince45.E
+ORDER, ERROR_ESTIMATOR_ORDER, N_STAGES = DormandPrince45.order, DormandPrince45.error_estimator_order, DormandPrince45.n_stages
+
+
 class CudaOdeOps:
-  """The float64 state ``y`` / ``y_new``, the stage derivatives ``K[7][n]`` and the float32 network input on the device.
-  ``drift(t, x32, k_out)`` (given by the sampler) evaluates the network on ``x32`` and writes the float64 drift.
+  """The float64 state ``y`` / ``y_new``, the stage derivatives ``K[n_stages + 1][n]`` and the float32 network input on
+  the device.  ``drift(t, x32, k_out)`` (given by the sampler) evaluates the network on ``x32`` and writes the float64
+  drift.  ``method`` is the controller class (a value of :data:`METHODS`) whose tableau the ops evaluate.
 
   ``extra`` > 0 appends that many zero-initialised float64 entries to the state (the likelihood ODE's ``logp`` slots,
-  ``likelihood.py:98``): ``x32`` is then the image part of the float32 stage state and ``k_out`` the whole stage row."""
+  ``likelihood.py:98``): ``x32`` is then the image part of the float32 stage state and ``k_out`` the whole stage row.
 
-  def __init__(self, x0, drift, extra=0):
+  Memory: n_stages + 3 float64 copies of the state plus one float32 copy.  For a CIFAR-10 likelihood state at batch 1024
+  (n = 1024 * 3072 + 1024 = 3,146,752 doubles, 25.2 MB each) that is 176 MB of stages for RK45 (7 rows), 101 MB for RK23
+  (4 rows) and 327 MB for DOP853 (13 rows); with y, y_new and x32 DOP853 holds 390 MB."""
+
+  def __init__(self, x0, drift, extra=0, method=DormandPrince45):
+    self.method = method
     self.device = x0.device
     self.shape = tuple(x0.shape)
     self.n_img = x0.numel()
@@ -141,7 +205,7 @@ class CudaOdeOps:
     self.n = y.numel()
     self.y = y.contiguous()
     self.y_new = torch.empty_like(self.y)
-    self.K = torch.empty(N_STAGES + 1, self.n, dtype=torch.float64, device=self.device)
+    self.K = torch.empty(method.n_stages + 1, self.n, dtype=torch.float64, device=self.device)
     self.x32_flat = torch.empty(self.n, dtype=torch.float32, device=self.device)
     self.x32 = self.x32_flat[:self.n_img].view(self.shape)
     self.ws = torch.zeros(int(_lib.load().b200_ode_workspace_doubles()), dtype=torch.float64, device=self.device)
@@ -149,7 +213,7 @@ class CudaOdeOps:
     self.host_reads = 0
 
   def _coefs(self, coefs):
-    arr = (ctypes.c_double * 8)()
+    arr = (ctypes.c_double * 16)()
     for j, c in enumerate(coefs):
       arr[j] = c
     return arr
@@ -165,9 +229,19 @@ class CudaOdeOps:
     return float(self.ws[0].item())          # the one device -> host scalar
 
   def error_sumsq(self, h, rtol, atol):
-    _lib.call('b200_ode_error_sumsq_f64', _lib.ptr(self.y), _lib.ptr(self.y_new), _lib.ptr(self.K), self.n, self._coefs(E),
-              len(E), float(h), float(rtol), float(atol), _lib.ptr(self.ws), _lib.stream_ptr(self.device))
+    e = self.method.E
+    _lib.call('b200_ode_error_sumsq_f64', _lib.ptr(self.y), _lib.ptr(self.y_new), _lib.ptr(self.K), self.n, self._coefs(e),
+              len(e), float(h), float(rtol), float(atol), _lib.ptr(self.ws), _lib.stream_ptr(self.device))
     return self._read()
+
+  def error_sumsq2(self, rtol, atol):
+    e5, e3 = self.method.E5, self.method.E3
+    _lib.call('b200_ode_error_sumsq2_f64', _lib.ptr(self.y), _lib.ptr(self.y_new), _lib.ptr(self.K), self.n,
+              self._coefs(e5), self._coefs(e3), len(e5), float(rtol), float(atol), _lib.ptr(self.ws),
+              _lib.stream_ptr(self.device))
+    self.host_reads += 1
+    s5, s3 = self.ws[:2].tolist()            # one device -> host copy of the two sums
+    return s5, s3
 
   def scaled_sumsq(self, slot, minus, rtol, atol):
     v = self.y if slot < 0 else self.K[slot]
@@ -178,7 +252,7 @@ class CudaOdeOps:
 
   def accept(self):
     self.y, self.y_new = self.y_new, self.y
-    self.K[0].copy_(self.K[N_STAGES])         # FSAL: self.f = f_new
+    self.K[0].copy_(self.K[self.method.n_stages])      # FSAL: self.f = f_new
 
   def state_f32(self):
     return self.y[:self.n_img].to(torch.float32).reshape(self.shape)

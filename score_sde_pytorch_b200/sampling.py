@@ -299,11 +299,14 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
                     method='RK45', eps=1e-3, device='cuda', device_solver=None):
   """Probability-flow ODE sampler (``sampling.py:414-485``): same signature, same ``(samples, nfe)`` result.
 
-  With an engine-backed network (NCSN++ or DDPM) on a CUDA device, ``method='RK45'`` and a stock VE / VP / sub-VP SDE the solve is
-  device-resident (``ode.py`` + ``csrc/ode.cu``): float64 state and Dormand-Prince stages in HBM, scipy's step-size
-  controller on the host, one double read back per attempted step.  Anything else - user models or SDEs, other
-  ``method`` values - runs the reference's host loop over ``scipy.integrate.solve_ivp`` (each right-hand side then
-  crosses PCIe twice, as in the reference).  ``device_solver=False`` forces the host loop (A/B and parity tests)."""
+  With an engine-backed network (NCSN++ or DDPM) on a CUDA device, an explicit Runge-Kutta ``method`` (``'RK23'``,
+  ``'RK45'`` or ``'DOP853'``) and a stock VE / VP / sub-VP SDE the solve is device-resident (``ode.py`` + ``csrc/ode.cu``):
+  float64 state and Runge-Kutta stages in HBM, scipy's step-size controller on the host, one transfer of the error sums
+  per attempted step.  Anything else - user models or SDEs, the implicit methods ``'Radau'``, ``'BDF'`` and ``'LSODA'``
+  (they need the Jacobian) - runs the reference's host loop over ``scipy.integrate.solve_ivp`` (each right-hand side then
+  crosses PCIe twice, as in the reference).  ``device_solver=False`` forces the host loop (A/B and parity tests);
+  ``device_solver=True`` requires the device solve (``NotImplementedError`` otherwise).  ``ode_sampler.last_stats``
+  records which solver ran and the method."""
 
   def denoise_update_fn(model, x):
     score_fn = get_score_fn(sde, model, train=False, continuous=True)
@@ -315,9 +318,16 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
     return sde.reverse(score_fn, probability_flow=True).sde(x, t)[0]
 
   def use_device_solver(model, x):
-    if device_solver is False or method != 'RK45' or not x.is_cuda:
+    from . import native, ode as _ode
+    if device_solver is False:
       return False
-    from . import native
+    if method not in _ode.METHODS:
+      if device_solver:
+        raise NotImplementedError(f'get_ode_sampler(device_solver=True): method {method!r} has no device solve '
+                                  f'(explicit Runge-Kutta methods only: {", ".join(_ode.METHODS)})')
+      return False
+    if not x.is_cuda:
+      return False
     from .models._engine import EngineModel
     ok = isinstance(native._unwrap(model), EngineModel) and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
     if device_solver and not ok:
@@ -331,10 +341,12 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
       if use_device_solver(model, x):
         from . import native, ode as _ode
         net = native._unwrap(model)
-        ops = _ode.CudaOdeOps(x.reshape(shape).to(torch.float32), _ode.engine_drift_fn(sde, net, shape[0], x.device))
-        nfe = _ode.DormandPrince45(ops, sde.T, eps, rtol=rtol, atol=atol).solve()
+        solver = _ode.METHODS[method]
+        ops = _ode.CudaOdeOps(x.reshape(shape).to(torch.float32), _ode.engine_drift_fn(sde, net, shape[0], x.device),
+                              method=solver)
+        nfe = solver(ops, sde.T, eps, rtol=rtol, atol=atol).solve()
         x = ops.state_f32()
-        ode_sampler.last_stats = dict(nfev=nfe, host_scalar_reads=ops.host_reads, solver='device')
+        ode_sampler.last_stats = dict(nfev=nfe, host_scalar_reads=ops.host_reads, solver='device', method=method)
       else:
         from scipy import integrate
 
@@ -347,7 +359,7 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
                                   rtol=rtol, atol=atol, method=method)
         x = torch.tensor(sol.y[:, -1]).reshape(shape).to(device).type(torch.float32)
         nfe = sol.nfev
-        ode_sampler.last_stats = dict(nfev=nfe, solver='scipy')
+        ode_sampler.last_stats = dict(nfev=nfe, solver='scipy', method=method)
       if denoise:
         x = denoise_update_fn(model, x)
       return inverse_scaler(x), nfe
