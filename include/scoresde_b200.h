@@ -115,7 +115,16 @@ typedef struct {
   int fir_taps;  float fir_kernel[8];   /* separable taps, e.g. {1,3,3,1} */
   int precision;                /* 0 = tensor cores on TF32-rounded fp32 operands where shapes allow, 1 = strict fp32
                                  * CUDA cores, 2 = tensor cores on fp16 operands (same 11-bit significand as TF32,
-                                 * fp32 accumulation; activations between layers stay fp32) */
+                                 * fp32 accumulation; activations between layers stay fp32), 3 = split TF32 ("3xTF32"):
+                                 * tensor cores on hi + lo pairs of TF32 values (hi = rna_tf32(x), lo = rna_tf32(x - hi)),
+                                 * three products per K step (lo*hi + hi*lo + hi*hi) into fp32 accumulators - close to fp32
+                                 * accuracy for about 3x the MMA work of 0.  Producers write fp32; a split pass in front of
+                                 * each tensor-core contraction makes the pairs of its activation operands ("split 3xtf32"
+                                 * ops), the weight blob holds a hi and a lo copy of every contraction weight (so
+                                 * b200_ncsnpp_weights_bytes is larger; the parameter table is that of precision 0).
+                                 * Attention runs as separate contractions, the few-channel levels of the nf = 16
+                                 * networks and the head on CUDA cores; contraction labels carry "3xtf32".  Other values
+                                 * are rejected by b200_ncsnpp_create. */
   int keep_activations;         /* debug: never recycle activation buffers so b200_ncsnpp_tap works */
   int lanes;                    /* 0/1: one plan over the whole batch (default); 2: two half-batch plans on two
                                  * streams (batches >= 128).  Off by default. */
@@ -154,7 +163,7 @@ typedef struct {
                                  * b200_ncsnpp_jvp: after each op its tangent op (the same contraction on the tangent buffers
                                  * without bias and time-embedding row, or a GroupNorm(+SiLU) / softmax tangent kernel).  Taken
                                  * by family 1 (DDPM) and by family 0 with naive_resample = 1, progressive = 0 and
-                                 * progressive_input = 0 (the DDPM++ configs), at precision 0 or 1 with lanes <= 1; anything
+                                 * progressive_input = 0 (the DDPM++ configs), at precision 0, 1 or 3 with lanes <= 1; anything
                                  * else is rejected by b200_ncsnpp_create.  A tangent plan runs attention as separate
                                  * contractions, the skip projections as their own contraction, and keeps the few-channel
                                  * levels on the CUDA-core kernel (op labels name the form). */

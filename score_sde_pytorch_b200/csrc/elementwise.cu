@@ -964,9 +964,11 @@ int launch_store_operand(const float* x, float* y, long long n, int mode, cudaSt
 
 // dst[tap*dt + o*dO + i] = src[o*so + i*si + tap*st]  (OIHW conv weights: so=I*R*S, si=R*S, st=1;
 // NIN W[in][out]: taps=1, so=1, si=out).  Default destination [tap][o][i] (dt=O*I, dO=I); the
-// flat-K packing of the input convolution uses dt=I, dO=row pitch.  Optional TF32 rounding.
+// flat-K packing of the input convolution uses dt=I, dO=row pitch.  Optional TF32 rounding; with `lo` (split TF32) dst
+// holds hi = rna_tf32(w) and lo, at the same index, rna_tf32(w - hi).
 __global__ void pack_weight_kernel(const float* __restrict__ src, float* __restrict__ dst, int taps, int O, int I,
-                                   long long so, long long si, long long stp, int round_out, long long dt, long long dO) {
+                                   long long so, long long si, long long stp, int round_out, long long dt, long long dO,
+                                   float* __restrict__ lo) {
   pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
   const long long total = (long long)taps * O * I;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
@@ -976,15 +978,40 @@ __global__ void pack_weight_kernel(const float* __restrict__ src, float* __restr
     const int o = (int)(t % O);
     const int tap = (int)(t / O);
     const float v = src[o * so + i * si + tap * stp];
-    store_operand1(dst, tap * dt + o * dO + i, v, round_out);
+    const long long d = tap * dt + o * dO + i;
+    store_operand1(dst, d, v, round_out);
+    if (lo) lo[d] = round_tf32(v - round_tf32(v));
   }
 }
 int launch_pack_weight(const float* src, float* dst, int taps, int O, int I, long long so, long long si,
-                       long long stp, int round_out, cudaStream_t st, long long dt, long long dO) {
+                       long long stp, int round_out, cudaStream_t st, long long dt, long long dO, float* lo) {
+  B200_REQUIRE(!lo || round_out == 1, "pack_weight: the split-TF32 lo copy goes with TF32-rounded weights");
   const long long total = (long long)taps * O * I;
   if (dt == 0) { dt = (long long)O * I; dO = I; }
-  launch_kernel(pack_weight_kernel, dim3((int)std::min<long long>((total + 255) / 256, 132LL * 16)), dim3(256), 0, st, 
-      src, dst, taps, O, I, so, si, stp, round_out, dt, dO);
+  launch_kernel(pack_weight_kernel, dim3((int)std::min<long long>((total + 255) / 256, 132LL * 16)), dim3(256), 0, st,
+      src, dst, taps, O, I, so, si, stp, round_out, dt, dO, lo);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+// split TF32 pair of an fp32 operand (precision 3): hi = rna_tf32(x), lo = rna_tf32(x - hi); x = hi + lo to ~2^-22 relative
+__global__ void __launch_bounds__(256) split_tf32_kernel(const float4* __restrict__ x, float4* __restrict__ hi,
+                                                         float4* __restrict__ lo, long long n4) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const float4 v = __ldg(x + i);
+    const float4 h = make_float4(round_tf32(v.x), round_tf32(v.y), round_tf32(v.z), round_tf32(v.w));
+    hi[i] = h;
+    lo[i] = make_float4(round_tf32(v.x - h.x), round_tf32(v.y - h.y), round_tf32(v.z - h.z), round_tf32(v.w - h.w));
+  }
+}
+int launch_split_tf32(const float* x, float* hi, float* lo, long long n, cudaStream_t st) {
+  B200_REQUIRE(n % 4 == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(hi) | reinterpret_cast<uintptr_t>(lo)) % 16) == 0,
+               "split_tf32: %lld elements / pointer alignment not float4-aligned", n);
+  const long long n4 = n / 4;
+  if (n4 == 0) return 0;
+  launch_kernel(split_tf32_kernel, dim3((int)std::min<long long>((n4 + 255) / 256, 132LL * 16)), dim3(256), 0, st,
+                reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(hi), reinterpret_cast<float4*>(lo), n4);
   B200_CHECK_LAUNCH();
   return 0;
 }
@@ -1027,17 +1054,17 @@ __global__ void __launch_bounds__(256) im2col3x3_nchw_kernel(const float* __rest
 #pragma unroll
     for (int q = 4; q < 8; ++q) *reinterpret_cast<uint4*>(row + 8 * q) = make_uint4(0u, 0u, 0u, 0u);
   } else {
-    float* row = patches + pg * 32;
+    float* row = patches + pg * 32;   // mode 1: TF32 grid; mode 0: fp32 as read (split TF32 plans split the patches after)
 #pragma unroll
     for (int q = 0; q < 8; ++q)
-      *reinterpret_cast<float4*>(row + 4 * q) = make_float4(round_tf32(v[4 * q]), round_tf32(v[4 * q + 1]), round_tf32(v[4 * q + 2]), round_tf32(v[4 * q + 3]));
+      store_operand4(row, 4 * q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]), mode);
   }
 }
 
 int launch_im2col3x3_nchw(const float* x, float* patches, int B, int C, int Hin, int Win, int H, int W, int stride,
                           int pad, int mode, cudaStream_t st) {
   B200_REQUIRE(C >= 1 && C <= 3, "im2col3x3: %d channels unsupported (1..3 image channels)", C);
-  B200_REQUIRE(mode == 1 || mode == 2, "im2col3x3: operand mode %d", mode);
+  B200_REQUIRE(mode >= 0 && mode <= 2, "im2col3x3: operand mode %d", mode);
   const long long total = (long long)B * H * W;
   const unsigned blocks = (unsigned)((total + 255) / 256);
   switch (C) {

@@ -27,7 +27,8 @@ struct Param {
   std::string name;
   int ndim; long long shape[4];
   long long off, count;      // location in the packed blob (floats)
-  int pack, taps, O, I, round;
+  int pack, taps, O, I, round;   // round: packed format (store_operand4 mode; 3 = split TF32, a hi and a lo copy)
+  long long lo = -1;             // split TF32: location of the lo copy (same packed layout as the hi copy at off)
 };
 
 struct Mod {
@@ -127,6 +128,7 @@ struct b200_ncsnpp {
   const float* in_v = nullptr; float* tout = nullptr;   // b200_ncsnpp_jvp: tangent direction and J v (tangent plans)
 
   const float* W(int pi) const { return wblob + params[pi].off; }
+  const float* Wlo(int pi) const { return params[pi].lo >= 0 ? wblob + params[pi].lo : nullptr; }   // split TF32 lo copy
   ~b200_ncsnpp() {
     for (auto* p : tcplans) tc_gemm_plan_destroy(p);
     for (auto* p : attnplans) tc_attn_plan_destroy(p);
@@ -145,8 +147,12 @@ int add_param(b200_ncsnpp* e, const std::string& name, std::vector<long long> sh
   p.count = 1;
   for (int i = 0; i < 4; ++i) { p.shape[i] = i < p.ndim ? shape[i] : 1; p.count *= p.shape[i]; }
   p.pack = pack; p.taps = taps; p.O = O; p.I = I; p.round = round;
-  if (fixed_off >= 0) p.off = fixed_off;
-  else { p.off = e->wcount; e->wcount += (std::max(p.count, reserve) + 63) & ~63LL; }
+  if (fixed_off >= 0) p.off = fixed_off;   // (split TF32: the caller places the lo copy)
+  else {
+    const long long n = (std::max(p.count, reserve) + 63) & ~63LL;
+    p.off = e->wcount; e->wcount += n;
+    if (round == 3) { p.lo = e->wcount; e->wcount += n; }
+  }
   e->params.push_back(p);
   return (int)e->params.size() - 1;
 }
@@ -164,7 +170,11 @@ TcGemmDesc tc_desc(const b200_ncsnpp* e, const float* a1, int C1, const float* a
 }
 
 // precision: 0 = tensor cores on TF32-grid fp32 operands, 1 = strict fp32 CUDA cores, 2 = tensor cores on fp16 operands
-// (same 11-bit significand as TF32, fp32 accumulation; half the operand bytes and twice the MMA rate)
+// (same 11-bit significand as TF32, fp32 accumulation; half the operand bytes and twice the MMA rate), 3 = split TF32
+// ("3xTF32"): tensor cores on hi / lo TF32 pairs of fp32 operands, three products per K step, close to fp32 accuracy.
+// In precision 3 producers write plain fp32 (as in precision 1); a split pass in front of each tensor-core contraction
+// writes the hi / lo pair of each activation operand, and the weight blob holds a hi and a lo copy of every contraction
+// weight.  The attention blocks run as separate contractions, the few-channel levels and the head on CUDA cores.
 bool tc_ok(const b200_ncsnpp* e, int C1, int C2, int Cout, int H, int W, int taps) {
   if (e->cfg.precision == 1) return false;
   return tc_gemm_supported(tc_desc(e, nullptr, C1, C2 ? (const float*)1 : nullptr, C2, H, W, 1, taps, nullptr, Cout), nullptr);
@@ -201,7 +211,8 @@ int build_graph(b200_ncsnpp* e) {
   }
   const int nf = c.nf, L = c.num_levels, nrb = c.num_res_blocks, ch = c.num_channels;
   const bool tcmode = c.precision != 1;
-  const int om = c.precision == 2 ? 2 : 1;      // operand store mode of tensor-core inputs (store_operand4)
+  // packed format of tensor-core weights (store_operand4 mode; 3: split TF32, a hi and a lo copy)
+  const int om = c.precision == 2 ? 2 : c.precision == 3 ? 3 : 1;
   const int flatk = om == 2 ? 64 : 32;          // elements of one 128-byte K step (im2col contraction depth)
   std::vector<int> all_res(L);
   for (int i = 0; i < L; ++i) all_res[i] = c.image_size >> i;
@@ -291,17 +302,19 @@ int build_graph(b200_ncsnpp* e) {
     // few tokens (T <= 64: the 4x4 block of CIFAR-10, the 8x8, 512-channel bottleneck of FFHQ-1024): one CTA per image
     // (attn_small_kernel); otherwise the block runs as separate contractions
     const bool small_ok = attn_small_supported(T, C);
-    m.tc0 = tcmode && (C % 128 == 0) && (m.tcattn || (small_ok && !c.tangent));   // q/k/v projections on tensor cores
-    // (tangent plans run every attention block as separate contractions: no small-token core, no fused core)
+    m.tc0 = tcmode && (C % 128 == 0) && (m.tcattn || (small_ok && !c.tangent && c.precision != 3));   // q/k/v projections on tensor cores
+    // (tangent and split-TF32 plans run every attention block as separate contractions: no small-token core, no fused core)
     m.gn0w = add_param(e, nm("GroupNorm_0.weight"), {C}, PK_COPY, 0, 0, 0, 0);
     m.gn0b = add_param(e, nm("GroupNorm_0.bias"), {C}, PK_COPY, 0, 0, 0, 0);
-    // q,k,v projection weights packed as one [3C][C] block (rows: q, k, v), biases as one [3C] vector
-    const long long wbase = e->wcount; e->wcount += 3LL * C * C;
-    const long long bbase = e->wcount; e->wcount += (3LL * C + 63) & ~63LL;
+    // q,k,v projection weights packed as one [3C][C] block (rows: q, k, v), biases as one [3C] vector; split TF32: the lo
+    // copies as a second [3C][C] block right after it
     const bool tcproj = m.tc0;
+    const long long wbase = e->wcount; e->wcount += 3LL * C * C * (tcproj && om == 3 ? 2 : 1);
+    const long long bbase = e->wcount; e->wcount += (3LL * C + 63) & ~63LL;
     for (int k = 0; k < 3; ++k) {
       m.nw[k] = add_param(e, nmi(m.index, "NIN_" + std::to_string(k) + ".W"), {C, C}, PK_NIN, 1, C, C, tcproj ? om : 0,
                           wbase + (long long)k * C * C / ((tcproj && om == 2) ? 2 : 1));   // fp16: the three blocks stay contiguous as [3C][C] halves
+      if (tcproj && om == 3) e->params[m.nw[k]].lo = wbase + 3LL * C * C + (long long)k * C * C;
       m.nb[k] = add_param(e, nmi(m.index, "NIN_" + std::to_string(k) + ".b"), {C}, PK_COPY, 0, 0, 0, 0, bbase + (long long)k * C);
     }
     m.tc2 = tc_ok(e, C, 0, C, res, res, 1) && (om != 2 || m.tcattn || T <= 64);   // output projection as a 1x1 conv over pixels
@@ -390,7 +403,8 @@ int build_graph(b200_ncsnpp* e) {
     // rows, as NCHW, divided by sigma.  2.3x faster than the CUDA-core head despite the 125 idle rows.
     // cfg.cuda_core_head = 1 keeps the head on CUDA cores with an fp32 input (it is the one convolution with no later
     // layer to average its operand rounding: +1e-4 of the parity budget on tensor cores).
-    m.tc0 = !c.cuda_core_head && tcmode && ch <= 32 && tc_ok(e, in_ch, 0, 128, c.image_size, c.image_size, 9) && (c.image_size * c.image_size) % 256 == 0 &&
+    // (split TF32 keeps the head on CUDA cores: strict fp32, no zero-padded pair of weight tiles)
+    m.tc0 = !c.cuda_core_head && tcmode && c.precision != 3 && ch <= 32 && tc_ok(e, in_ch, 0, 128, c.image_size, c.image_size, 9) && (c.image_size * c.image_size) % 256 == 0 &&
             (c.image_size <= 128 || c.image_size % 128 == 0);
     m.w = m.tc0 ? add_param(e, nm("weight"), {ch, in_ch, 3, 3}, PK_CONV_PAD128, 9, ch, in_ch, om, -1, 9LL * 128 * in_ch)
                 : add_param(e, nm("weight"), {ch, in_ch, 3, 3}, PK_CONV, 9, ch, in_ch, 0);
@@ -436,7 +450,8 @@ struct Builder {
   bool fused_stats = false;
   bool lowc_gn = false;                        // the few-channel convolutions (conv_lowc.cu, TF32 mode) apply GroupNorm+SiLU while staging their input
   int lane = 0;                                // which half-batch plan this builder fills (ops or ops2)
-  int om = 1;                                  // operand store mode of tensor-core inputs: 1 TF32-grid fp32, 2 fp16
+  int om = 1;                                  // operand store mode of tensor-core inputs: 1 TF32-grid fp32, 2 fp16, 0 fp32 (split TF32)
+  bool split = false;                          // split TF32 (precision 3): contractions read hi / lo pairs made by split_pair()
   std::string next_name;                       // label of the next op (shape summary for the per-op profile)
   double next_bytes = 0.0;                     // algorithmic HBM bytes of the next op
   bool tan = false;                            // tangent plan (cfg.tangent): every tensor carries its tangent in Tensor::d
@@ -450,7 +465,8 @@ struct Builder {
   }
   Builder(b200_ncsnpp* e_, int B_, char* base_, bool dry_, int lane_ = 0) : e(e_), B(B_), base(base_), dry(dry_), arena(e_->cfg.keep_activations != 0), lane(lane_) {
     fused_stats = e_->cfg.precision != 1;
-    om = e_->cfg.precision == 2 ? 2 : 1;
+    split = e_->cfg.precision == 3;
+    om = e_->cfg.precision == 2 ? 2 : split ? 0 : 1;
     tan = e_->cfg.tangent != 0;
     lowc_gn = e_->cfg.precision == 0 && e_->cfg.separate_groupnorm != 2 && !tan;
     if (dry_) stats_base = reinterpret_cast<char*>(uintptr_t(1) << 40);   // any non-null base: only offsets matter in a dry run
@@ -484,6 +500,24 @@ struct Builder {
     return p;
   }
   void ffree(float* p, long long bytes) { arena.release((char*)p - base, bytes); }
+
+  // split TF32: hi = rna_tf32(x) and lo = rna_tf32(x - hi) of the n fp32 elements at x, one split pass into a temporary
+  // [hi | lo] buffer.  The caller releases it once the contraction that reads it is planned (later ops, which may reuse
+  // the memory, run after that contraction).
+  struct Pair { const float* hi = nullptr; const float* lo = nullptr; float* buf = nullptr; long long bytes = 0; };
+  Pair split_pair(const float* x, long long n, const char* what) {
+    Pair s;
+    if (!x) return s;
+    if (n % 4) { set_error("ncsnpp: split TF32 operand of %lld elements (not a multiple of 4)", n); rc = 2; return s; }
+    s.buf = falloc(2 * n, &s.bytes);
+    float* hi = s.buf; float* lo = s.buf + n;
+    s.hi = hi; s.lo = lo;
+    name("split 3xtf32 %s", what);
+    next_bytes = n * 12.0;
+    op(1, [=](cudaStream_t st) { return launch_split_tf32(x, hi, lo, n, st); }, 6);
+    return s;
+  }
+  void release(Pair& s) { if (s.buf) ffree(s.buf, s.bytes); s = Pair(); }
 
   // kind: 0 tensor-core contraction, 1 CUDA-core contraction, 2 GroupNorm, 3 FIR, 4 softmax, 5 time embedding, 6 misc
   void op(int launches, std::function<int(cudaStream_t)> f, int kind = 6, double flops = 0.0) {
@@ -648,6 +682,20 @@ struct Builder {
       }
       if (o.stats_ && fused_stats && (ep.rows_per_img % 32 == 0 || ep.rows_per_img == 16)) { out.qs = qalloc(Cout); d.qstats = out.qs; }
       d.epi = ep;
+      if (split) {   // every activation operand as a hi / lo pair, the weights' lo copies from the blob
+        const Tensor* src[4] = {&a1, &a2, &x3, &x4};
+        Pair pr[4];
+        for (int s = 0; s < 4; ++s) {
+          const Tensor& t = *src[s];
+          pr[s] = split_pair(t.p, (long long)B * t.H * t.W * t.C, s < 2 ? "conv input" : "skip input");
+        }
+        if (rc) return;
+        d.split = 1;
+        d.a1 = pr[0].hi; d.a1_lo = pr[0].lo; d.a2 = pr[1].hi; d.a2_lo = pr[1].lo;
+        d.a3 = pr[2].hi; d.a3_lo = pr[2].lo; d.a4 = pr[3].hi; d.a4_lo = pr[3].lo;
+        d.w_lo = e->Wlo(pw); d.w2_lo = x3.p ? e->Wlo(o.skip_w_) : nullptr;
+        for (auto& q : pr) release(q);
+      }
       if (dry) return;
       TcGemmPlan* pl = nullptr;
       if (int r = tc_gemm_plan_create(d, &pl)) { rc = r; return; }
@@ -656,7 +704,7 @@ struct Builder {
            x3.p ? " +skipproj" : "", residual ? " +res" : "", tc_gemm_form(pl));
       if (x3.p) next_name += " " + std::to_string(x3.C + x4.C);
       {
-        const double es = om == 2 ? 2.0 : 4.0, px = (double)B * out.H * out.W;
+        const double es = om == 2 ? 2.0 : split ? 8.0 : 4.0, px = (double)B * out.H * out.W;   // split TF32: hi + lo
         const double in_px = (double)B * (Hin ? (double)Hin * Hin : (double)out.H * out.W);
         next_bytes = in_px * (a1.C + a2.C) * es + px * (x3.C + x4.C) * es + px * Cout * (o.round_ == 2 ? 2.0 : 4.0) +
                      (residual ? px * Cout * 4.0 : 0.0) + ((double)taps * (a1.C + a2.C) + x3.C + x4.C) * Cout * es;
@@ -672,8 +720,8 @@ struct Builder {
       s.epi = ep;
       // few-channel levels of the nf = 16 networks: warp-level TF32 MMAs keep them at the HBM roofline (conv_lowc.cu);
       // strict-fp32 mode and every other shape stay on the CUDA-core kernel
-      // (tangent plans keep every level on the CUDA-core kernel)
-      const bool lowc = e->cfg.precision != 1 && !tan && !a1.f16 && !a2.f16 && sumC % 2 == 0 && conv_lowc_supported(s);
+      // (tangent and split-TF32 plans keep every level on the CUDA-core kernel)
+      const bool lowc = e->cfg.precision != 1 && !split && !tan && !a1.f16 && !a2.f16 && sumC % 2 == 0 && conv_lowc_supported(s);
       if (o.stats_ && lowc && fused_stats) { out.qs = qalloc(Cout); s.qstats = out.qs; }   // the epilogue sums what the next GroupNorm needs
       if (o.gn_) {
         if (!lowc) { set_error("ncsnpp: GroupNorm on load planned for a convolution the few-channel kernel does not take"); rc = 2; return; }
@@ -690,11 +738,12 @@ struct Builder {
     }
   }
 
-  // batched C[b] = A[b] * W[b]^T
+  // batched C[b] = A[b] * W[b]^T.  Split TF32: a_lo / w_lo are the lo twins of A / W when the caller has them (weights, an
+  // operand split once for two products); a null twin makes this contraction split its operand itself.
   void gemm(bool use_tc, const float* A, long long lda, long long a_rows, int a_batch_rows, const float* Wm, long long ldw,
             long long w_rows, int w_batch_rows, int nbatch, int M, int N, int K, const float* bias,
             const float* residual, long long ld_res, float scale, int round, float* out, long long ldo,
-            double* qstats = nullptr, int rows_per_img = 1 << 30) {
+            double* qstats = nullptr, int rows_per_img = 1 << 30, const float* a_lo = nullptr, const float* w_lo = nullptr) {
     Epilogue ep; memset(&ep, 0, sizeof(ep));
     ep.bias = bias; ep.residual = residual; ep.ld_res = ld_res; ep.scale = scale; ep.round_tf32 = round;
     ep.rows_per_img = rows_per_img; ep.out = out; ep.ld_out = ldo;
@@ -702,13 +751,21 @@ struct Builder {
       TcGemmDesc d = tc_desc(e, A, K, nullptr, 0, 0, 0, 0, 1, Wm, N);
       d.conv = 0; d.a_rows = a_rows; d.a_ld = lda; d.a_batch_rows = a_batch_rows;
       d.w_rows = w_rows; d.w_ld = ldw; d.w_batch_rows = w_batch_rows; d.nbatch = nbatch; d.M_per_batch = M; d.qstats = qstats; d.epi = ep;
+      if (split) {   // the rows the contraction reads: (rows - 1) pitches + K elements from the base
+        Pair pa, pw;
+        if (!a_lo) { pa = split_pair(A, (a_rows - 1) * lda + K, "gemm A"); d.a1 = pa.hi; a_lo = pa.lo; }
+        if (!w_lo) { pw = split_pair(Wm, (w_rows - 1) * ldw + K, "gemm W"); d.w = pw.hi; w_lo = pw.lo; }
+        if (rc) return;
+        d.split = 1; d.a1_lo = a_lo; d.w_lo = w_lo;
+        release(pa); release(pw);
+      }
       if (dry) return;
       TcGemmPlan* pl = nullptr;
       if (int r = tc_gemm_plan_create(d, &pl)) { rc = r; return; }
       e->tcplans.push_back(pl);
       name("gemm %dx(%dx%dx%d)%s [%s]", nbatch, M, N, K, residual ? " +res" : "", tc_gemm_form(pl));
       {
-        const double es = om == 2 ? 2.0 : 4.0;
+        const double es = om == 2 ? 2.0 : split ? 8.0 : 4.0;
         next_bytes = (double)(a_batch_rows ? nbatch : 1) * M * K * es + (double)(w_batch_rows ? nbatch : 1) * N * K * es +
                      (double)nbatch * M * N * (round == 2 ? 2.0 : 4.0) + (residual ? (double)nbatch * M * N * 4.0 : 0.0);
       }
@@ -853,9 +910,10 @@ struct Builder {
       twin([&](bool d) {   // tangent: dq, dk, dv, the projections of da without bias
         // q,k = a Wq^T + bq | a Wk^T + bk   (layerspp.py:78-79) in one N=2C contraction
         gemm(tc, d ? a.d : a.p, C, BT, 0 /* rows enumerated flat */, Wqkv, C, 2LL * C, 0, 1, (int)BT, 2 * C, C, d ? nullptr : bqkv,
-             nullptr, 0, 1.f, tc ? om : 0, d ? dqk : qk, 2 * C);
+             nullptr, 0, 1.f, tc ? om : 0, d ? dqk : qk, 2 * C, nullptr, 1 << 30, nullptr, e->Wlo(m.nw[0]));
         // v^T[b][c][t] = sum_i Wv[c][i] a[b][t][i]   (bias bv is added after the PV product: softmax rows sum to 1)
-        gemm(tc, wv, C, C, 0, d ? a.d : a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, d ? dvT : vT, T, nullptr, 1 << 30);
+        gemm(tc, wv, C, C, 0, d ? a.d : a.p, C, BT, T, B, C, T, C, nullptr, nullptr, 0, 1.f, tc ? om : 0, d ? dvT : vT, T, nullptr, 1 << 30,
+             e->Wlo(m.nw[0]) ? e->Wlo(m.nw[0]) + 2LL * C * C : nullptr);
       });
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
@@ -863,7 +921,7 @@ struct Builder {
       if (om == 2 && !(tc && m.tc2 && tc_attn_supported(T, C))) {
         set_error("ncsnpp: fp16 operand mode needs the fused attention core (T=%d C=%d)", T, C); rc = 2; return Tensor();
       }
-      if (tc && m.tc2 && tc_attn_supported(T, C) && !tan) {
+      if (tc && m.tc2 && tc_attn_supported(T, C) && !tan && !split) {
         Tensor out = talloc(C, x.H, x.W);
         if (fused_stats) out.qs = qalloc(C);
         if (!dry) {
@@ -881,8 +939,13 @@ struct Builder {
         return out;
       }
       float* S = falloc2(BT * T, &sb, &dS);
-      // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax
-      gemm(tc, qk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30);
+      // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax (split TF32: q | k split once for both operands)
+      Pair qkp;
+      if (tc && split) qkp = split_pair(qk, (long long)B * T * 2 * C, "q|k");
+      const float* qkh = qkp.hi ? qkp.hi : qk;
+      gemm(tc, qkh, 2 * C, BT, T, qkh + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30,
+           qkp.lo, qkp.lo ? qkp.lo + C : nullptr);
+      release(qkp);
       if (tan) {   // dS = dq k^T + q dk^T
         long long tb; float* t1 = falloc(BT * T, &tb);
         tangent([&] {
@@ -893,19 +956,20 @@ struct Builder {
       }
       ffree(qk, qkb);
       name("softmax T=%d", T);
-      op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4);
+      const int prnd = tc ? om : 0;   // probabilities in the operand format of the P.V contraction (fp32 when split TF32)
+      op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, prnd, st); }, 4);
       if (tan) {   // dP = P (sc dS - rowsum(P sc dS)), over dS
         name("softmax_tangent T=%d", T);
-        tangent([&] { op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, tc ? 1 : 0, st); }, 4); });
+        tangent([&] { op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, prnd, st); }, 4); });
       }
       O = falloc2(BT * C, &ob, &dO);
       // h[b][q][c] = sum_k P[q][k] v[k][c] + bv[c]   (layerspp.py:86)
-      gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? 1 : 0, O, C);
+      gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? om : 0, O, C);
       if (tan) {   // dO = dP v + P dv
         long long tb; float* t2 = falloc(BT * C, &tb);
         tangent([&] {
           gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
-          gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? 1 : 0, dO, C);
+          gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? om : 0, dO, C);
         });
         ffree(t2, tb);
       }
@@ -924,7 +988,9 @@ struct Builder {
   Tensor downsample(const Mod& m, Tensor& x) {
     const int H = x.H, Ho = H / 2;
     Tensor out = talloc(m.cout, Ho, Ho);
-    if (m.tc0) {
+    if (m.tc0 && split) {
+      conv(true, x, Tensor(), m.w, m.b, out, Conv().stats().stride(2, H));   // the contraction's split pass reads the fp32 block output
+    } else if (m.tc0) {
       // the block output is fp32; the tensor cores read it in the operand format (TF32 grid / fp16)
       Tensor xo = talloc(x.C, H, H);
       const long long n = (long long)B * H * H * x.C; const int omc = om;
@@ -1263,6 +1329,8 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
   B200_REQUIRE(cfg->separate_groupnorm != 0, "ncsnpp_create: separate_groupnorm = 0 (GroupNorm applied on load by the tensor-core "
                "convolution) is not available in this build; use 1 or 2");
   B200_REQUIRE(cfg->family == 0 || cfg->family == 1, "ncsnpp_create: family=%d unknown (0 NCSN++, 1 DDPM)", cfg->family);
+  B200_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, "ncsnpp_create: precision=%d unknown (0 tf32, 1 fp32, 2 f16, 3 split tf32)",
+               cfg->precision);
   if (cfg->family == 1) {
     B200_REQUIRE(cfg->conditional, "ncsnpp_create: DDPM (family 1) needs conditional = 1 (the reference's own constructor fails "
                  "without time conditioning, models/ddpm.py:58-71)");
@@ -1273,8 +1341,8 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
     // the forward-mode tangent pass (b200_ncsnpp_jvp) covers DDPM and the DDPM++ family; everything else is refused here
     // rather than approximated
     B200_REQUIRE(cfg->tangent == 1, "ncsnpp_create: tangent=%d unknown (0 or 1)", cfg->tangent);
-    B200_REQUIRE(cfg->precision == 0 || cfg->precision == 1, "ncsnpp_create: tangent = 1 with precision = %d: the tangent pass "
-                 "runs in precision 0 (tf32) or 1 (fp32), not on fp16 operands", cfg->precision);
+    B200_REQUIRE(cfg->precision != 2, "ncsnpp_create: tangent = 1 with precision = %d: the tangent pass "
+                 "runs in precision 0 (tf32), 1 (fp32) or 3 (split tf32), not on fp16 operands", cfg->precision);
     B200_REQUIRE(cfg->lanes <= 1, "ncsnpp_create: tangent = 1 with lanes = %d: the tangent pass runs one lane", cfg->lanes);
     if (cfg->family == 0) {
       B200_REQUIRE(cfg->naive_resample, "ncsnpp_create: tangent = 1 with naive_resample = 0: FIR resampling has no tangent pass");
@@ -1331,14 +1399,17 @@ int b200_ncsnpp_load_param(b200_ncsnpp_t* h, int index, const float* src, void* 
     B200_CHECK_CUDA(cudaMemcpyAsync(dst, src, p.count * 4, cudaMemcpyDeviceToDevice, st));
     return 0;
   }
+  // split TF32 (round 3): the hi copy on the TF32 grid at off, the lo copy in the same layout at p.lo
+  const int rnd = p.round == 3 ? 1 : p.round;
+  float* lo = p.round == 3 ? h->wblob + p.lo : nullptr;
   if (p.pack == PK_CONV_FLAT32)   // OIHW (3x3, I*9 <= 32) -> [O][32] with k = tap*I + i (rest of the row stays zero)
-    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, p.round, st, p.I, p.round == 2 ? 64 : 32);
+    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, rnd, st, p.I, p.round == 2 ? 64 : 32, lo);
   if (p.pack == PK_CONV_PAD128)   // OIHW -> [tap][128][I], rows >= O stay zero
-    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, p.round, st, 128LL * p.I, p.I);
+    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, rnd, st, 128LL * p.I, p.I, lo);
   if (p.pack == PK_CONV)   // OIHW -> [tap][O][I]
-    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, p.round, st);
+    return launch_pack_weight(src, dst, p.taps, p.O, p.I, (long long)p.I * p.taps, p.taps, 1, rnd, st, 0, 0, lo);
   // NIN W[in][out] -> [out][in]
-  return launch_pack_weight(src, dst, 1, p.O, p.I, 1, p.O, 0, p.round, st);
+  return launch_pack_weight(src, dst, 1, p.O, p.I, 1, p.O, 0, rnd, st, 0, 0, lo);
 }
 
 namespace {

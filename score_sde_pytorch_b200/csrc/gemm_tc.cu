@@ -6,7 +6,9 @@
 //
 // Operands are written by their producers in the contraction's format: fp32 bit patterns rounded to the TF32 grid
 // (wgmma .tf32, 32 channels per 128-byte K step) or IEEE fp16 (wgmma .f16, 64 channels per K step); either way 11
-// significand bits, fp32 accumulation in registers.
+// significand bits, fp32 accumulation in registers.  Split TF32 (precision 3, "3xTF32") gives every operand a lo twin
+// (x = hi + lo, both on the TF32 grid) and walks each K step three times - A lo x W hi, A hi x W lo, A hi x W hi - into
+// the same accumulator: only the producer's tensor-map choice and the K count change; ring, barriers and epilogue do not.
 //
 // Kernels (persistent, warp-specialised, 384 threads):
 //   gemm_tc_kernel<BN>   one CTA per tile: 128 rows x BN columns, or - `swap` - 128 output channels x 256 pixels
@@ -50,7 +52,10 @@ struct TcParams {
   CUtensorMap tmA1, tmA2, tmW;
   CUtensorMap tmA3, tmA4, tmW2;            // optional extra 1x1 K phase (fused skip projection): out += [A3|A4] W2^T
   CUtensorMap tmH1, tmH2;                  // halo form: box = [bke channels, W, tile rows + 2, 1] of the two filter sources
-  int halo;                                // 1: 3x3 taps read W-shifted halo copies of the tile (3 loads per channel chunk instead of 9)
+  // split TF32: the same maps over the lo twins of every operand (copies of the hi maps otherwise)
+  CUtensorMap tmA1l, tmA2l, tmWl, tmA3l, tmA4l, tmW2l, tmH1l, tmH2l;
+  int nphase;                              // 3: split TF32, every K step loads (A lo, W hi), (A hi, W lo), (A hi, W hi); else 1
+  int halo;                               // 1: 3x3 taps read W-shifted halo copies of the tile (3 loads per channel chunk instead of 9)
   int halo_dh_bytes;                       // W * 128: bytes between the operand windows of consecutive filter rows inside a copy
   int halo_copy_bytes;                     // (tile rows + 2) * W * 128: bytes of one halo copy
   int halo_prefetch;                       // 1: the halo producers prefetch the next tile's halo boxes (all channel chunks) into L2 (opt-in: measured -2 %)
@@ -290,7 +295,7 @@ template <int BN, bool F16>
 __device__ __forceinline__ void gemm_tc_consumer(const TcParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                                  uint64_t* wfull_bar, uint64_t* wempty_bar, int g, int wq, int lane) {
   using L = SmemLayout<BN>;
-  const int kiters = (p.kchunks1 + p.kchunks2) * p.taps + p.kchunks3 + p.kchunks4;
+  const int kiters = ((p.kchunks1 + p.kchunks2) * p.taps + p.kchunks3 + p.kchunks4) * p.nphase;
   const Epilogue& e = p.epi;
   uint32_t stage = 0, phase = 0, ws = 0, wphase = 0;
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -302,7 +307,7 @@ __device__ __forceinline__ void gemm_tc_consumer(const TcParams& p, uint8_t* sme
       int it = 0, pend_ws = -1, pend_x = -1;
       for (int src = 0; src < 4; ++src) {
         const int nch = src == 0 ? p.kchunks1 : src == 1 ? p.kchunks2 : src == 2 ? p.kchunks3 : p.kchunks4;
-        const int ncopies = src < 2 ? 3 * nch : nch, ntap = src < 2 ? 3 : 1;
+        const int ncopies = (src < 2 ? 3 * nch : nch) * p.nphase, ntap = src < 2 ? 3 : 1;
         for (int c = 0; c < ncopies; ++c) {
           mbar_wait(&full_bar[stage], phase);
           const uint32_t sx = smem_u32(smem + stage * HALO_X_BYTES);
@@ -419,6 +424,7 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
     if (warp != 0) return;
     // ======================= TMA producer (whole warp; one elected lane issues, see elect_one) =======================
     const bool issue = elect_one();
+    const int alo_ph = p.nphase == 3 ? 0 : -1;   // split TF32: the product phase that reads the pixel / row operand's lo twin
     uint32_t stage = 0, phase = 0;
     if (BN == 256 && p.halo) {
       // halo form (swapped operands, one image per 256-pixel tile, W <= 32): per channel chunk three halo copies, each
@@ -442,40 +448,46 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
           const int wcol0 = src == 1 ? p.C1 : src == 3 ? p.C3 : 0;
           for (int kc = 0; kc < nch; ++kc) {
             if (src < 2) {
-              const CUtensorMap* tmH = src == 0 ? &p.tmH1 : &p.tmH2;
               for (int dwi = 0; dwi < 3; ++dwi) {
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                if (issue) {
-                  mbar_expect_tx(&full_bar[stage], (uint32_t)p.halo_copy_bytes);
-                  tma_load_4d(tmH, smem + stage * HALO_X_BYTES, &full_bar[stage], kc * bke, dwi - 1, h0 - 1, img0);
-                }
-                if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
-                for (int dhi = 0; dhi < 3; ++dhi) {
-                  mbar_wait(&wempty_bar[ws], wphase ^ 1);
+                // split TF32: the copy + its three weight slices once per product (pixels lo / hi / hi, weights hi / lo / hi)
+                for (int ph = 0; ph < p.nphase; ++ph) {
+                  const CUtensorMap* tmH = ph == alo_ph ? (src == 0 ? &p.tmH1l : &p.tmH2l) : (src == 0 ? &p.tmH1 : &p.tmH2);
+                  const CUtensorMap* tmW = ph == 1 ? &p.tmWl : &p.tmW;
+                  mbar_wait(&empty_bar[stage], phase ^ 1);
                   if (issue) {
-                    mbar_expect_tx(&wfull_bar[ws], A_STAGE_BYTES);
-                    tma_load_2d(&p.tmW, wring + ws * A_STAGE_BYTES, &wfull_bar[ws], wcol0 + kc * bke, wrow0 + (dhi * 3 + dwi) * p.N_total);
+                    mbar_expect_tx(&full_bar[stage], (uint32_t)p.halo_copy_bytes);
+                    tma_load_4d(tmH, smem + stage * HALO_X_BYTES, &full_bar[stage], kc * bke, dwi - 1, h0 - 1, img0);
                   }
-                  if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
+                  if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
+                  for (int dhi = 0; dhi < 3; ++dhi) {
+                    mbar_wait(&wempty_bar[ws], wphase ^ 1);
+                    if (issue) {
+                      mbar_expect_tx(&wfull_bar[ws], A_STAGE_BYTES);
+                      tma_load_2d(tmW, wring + ws * A_STAGE_BYTES, &wfull_bar[ws], wcol0 + kc * bke, wrow0 + (dhi * 3 + dwi) * p.N_total);
+                    }
+                    if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
+                  }
                 }
               }
             } else {
               // extra 1x1 phase (fused skip projection): the plain 256-pixel tile as two 128-pixel boxes, its own weights
-              const CUtensorMap* tmA = src == 2 ? &p.tmA3 : &p.tmA4;
               const int h1 = h0 + 128 / p.W;
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              if (issue) {
-                mbar_expect_tx(&full_bar[stage], 2 * A_STAGE_BYTES);
-                tma_load_4d(tmA, smem + stage * HALO_X_BYTES, &full_bar[stage], kc * bke, 0, h0, img0);
-                tma_load_4d(tmA, smem + stage * HALO_X_BYTES + A_STAGE_BYTES, &full_bar[stage], kc * bke, 0, h1, img0);
+              for (int ph = 0; ph < p.nphase; ++ph) {
+                const CUtensorMap* tmA = ph == alo_ph ? (src == 2 ? &p.tmA3l : &p.tmA4l) : (src == 2 ? &p.tmA3 : &p.tmA4);
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                if (issue) {
+                  mbar_expect_tx(&full_bar[stage], 2 * A_STAGE_BYTES);
+                  tma_load_4d(tmA, smem + stage * HALO_X_BYTES, &full_bar[stage], kc * bke, 0, h0, img0);
+                  tma_load_4d(tmA, smem + stage * HALO_X_BYTES + A_STAGE_BYTES, &full_bar[stage], kc * bke, 0, h1, img0);
+                }
+                if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
+                mbar_wait(&wempty_bar[ws], wphase ^ 1);
+                if (issue) {
+                  mbar_expect_tx(&wfull_bar[ws], A_STAGE_BYTES);
+                  tma_load_2d(ph == 1 ? &p.tmW2l : &p.tmW2, wring + ws * A_STAGE_BYTES, &wfull_bar[ws], wcol0 + kc * bke, wrow0);
+                }
+                if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
               }
-              if (++stage == HALO_XS) { stage = 0; phase ^= 1; }
-              mbar_wait(&wempty_bar[ws], wphase ^ 1);
-              if (issue) {
-                mbar_expect_tx(&wfull_bar[ws], A_STAGE_BYTES);
-                tma_load_2d(&p.tmW2, wring + ws * A_STAGE_BYTES, &wfull_bar[ws], wcol0 + kc * bke, wrow0);
-              }
-              if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
             }
           }
         }
@@ -506,8 +518,10 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
       for (int src = 0; src < 4; ++src) {
         const int nch = src == 0 ? p.kchunks1 : src == 1 ? p.kchunks2 : src == 2 ? p.kchunks3 : p.kchunks4;
         if (nch == 0) continue;
-        const CUtensorMap* tmA = src == 0 ? &p.tmA1 : src == 1 ? &p.tmA2 : src == 2 ? &p.tmA3 : &p.tmA4;
-        const CUtensorMap* tmW = src < 2 ? &p.tmW : &p.tmW2;
+        const CUtensorMap* tmAh = src == 0 ? &p.tmA1 : src == 1 ? &p.tmA2 : src == 2 ? &p.tmA3 : &p.tmA4;
+        const CUtensorMap* tmWh = src < 2 ? &p.tmW : &p.tmW2;
+        const CUtensorMap* tmAl = src == 0 ? &p.tmA1l : src == 1 ? &p.tmA2l : src == 2 ? &p.tmA3l : &p.tmA4l;
+        const CUtensorMap* tmWl = src < 2 ? &p.tmWl : &p.tmW2l;
         const int wcol0 = src == 1 ? p.C1 : src == 3 ? p.C3 : 0;
         const int ntaps = src < 2 ? p.taps : 1;
         // K order.  Default: filter tap, then channel chunk - consecutive loads sweep the channel vector of the same shifted
@@ -520,23 +534,27 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
             const int kc = p.chunk_major ? o : i, t = p.chunk_major ? i : o;
             const int tap = (ntaps == 1 || !p.chunk_major) ? t : (t % p.S) * p.S + t / p.S;
             const int dh = src < 2 ? tap / p.S - p.pad : 0, dw = src < 2 ? tap % p.S - p.pad : 0;
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * L::STAGE_BYTES;
-            uint8_t* sb = sa + A_STAGE_BYTES;
-            if (issue) {
-              mbar_expect_tx(&full_bar[stage], L::STAGE_BYTES);
-              if (p.swap) {
-                // first 16 KiB: 128 output channels x 32 k of W (MMA A); next 32 KiB: 256 pixels x 32 k (MMA B)
-                tma_load_2d(tmW, sa, &full_bar[stage], wcol0 + kc * bke, wrow0 + tap * p.N_total);
-                tma_load_4d(tmA, sb, &full_bar[stage], kc * bke, w0 + dw, h0 + dh, img0);
-                tma_load_4d(tmA, sb + A_STAGE_BYTES, &full_bar[stage], kc * bke, w1 + dw, h1 + dh, img1);
-              } else {
-                if (p.conv) tma_load_4d(tmA, sa, &full_bar[stage], kc * bke, w0 * p.stride + dw, h0 * p.stride + dh, img0);
-                else tma_load_4d(tmA, sa, &full_bar[stage], kc * bke, arow0, 0, 0);
-                tma_load_2d(tmW, sb, &full_bar[stage], wcol0 + kc * bke, wrow0 + tap * p.N_total);
+            for (int ph = 0; ph < p.nphase; ++ph) {   // split TF32: (A lo, W hi), (A hi, W lo), (A hi, W hi)
+              const CUtensorMap* tmA = ph == alo_ph ? tmAl : tmAh;
+              const CUtensorMap* tmW = ph == 1 ? tmWl : tmWh;
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              uint8_t* sa = smem + stage * L::STAGE_BYTES;
+              uint8_t* sb = sa + A_STAGE_BYTES;
+              if (issue) {
+                mbar_expect_tx(&full_bar[stage], L::STAGE_BYTES);
+                if (p.swap) {
+                  // first 16 KiB: 128 output channels x 32 k of W (MMA A); next 32 KiB: 256 pixels x 32 k (MMA B)
+                  tma_load_2d(tmW, sa, &full_bar[stage], wcol0 + kc * bke, wrow0 + tap * p.N_total);
+                  tma_load_4d(tmA, sb, &full_bar[stage], kc * bke, w0 + dw, h0 + dh, img0);
+                  tma_load_4d(tmA, sb + A_STAGE_BYTES, &full_bar[stage], kc * bke, w1 + dw, h1 + dh, img1);
+                } else {
+                  if (p.conv) tma_load_4d(tmA, sa, &full_bar[stage], kc * bke, w0 * p.stride + dw, h0 * p.stride + dh, img0);
+                  else tma_load_4d(tmA, sa, &full_bar[stage], kc * bke, arow0, 0, 0);
+                  tma_load_2d(tmW, sb, &full_bar[stage], wcol0 + kc * bke, wrow0 + tap * p.N_total);
+                }
               }
+              if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
@@ -632,6 +650,9 @@ bool tc_gemm_supported(const TcGemmDesc& d, const char** why) {
   if ((d.qstats || d.epi.rowvec) && !(d.epi.rows_per_img % 32 == 0 || d.epi.rows_per_img == 16)) return fail("per-image epilogue terms need rows_per_img % 32 == 0 or == 16");
   if (d.epi.ld_out % 4 || (d.epi.residual && d.epi.ld_res % 4)) return fail("output pitch must be a multiple of 4 elements");
   if (d.epi.round_tf32 == 2 && d.epi.ld_out % 8) return fail("fp16 output pitch must be a multiple of 8 elements");
+  if (d.split && d.f16) return fail("split TF32 takes TF32 operands, not fp16");
+  if (d.split && (!d.a1_lo || (d.a2 && !d.a2_lo) || (d.a3 && !d.a3_lo) || (d.a4 && !d.a4_lo) || !d.w_lo || (d.a3 && !d.w2_lo)))
+    return fail("split TF32 needs the lo twin of every operand");
   return true;
 }
 
@@ -647,8 +668,16 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
   p.S = d.taps == 9 ? 3 : 1; p.pad = (d.taps == 9 && !d.valid_pad) ? 1 : 0;
   p.stride = d.stride == 2 ? 2 : 1;
   p.f16 = d.f16 ? 1 : 0;
+  p.nphase = d.split ? 3 : 1;
 
   const bool f16 = d.f16 != 0;
+  // every map is encoded over the hi operand and, in split-TF32 plans, once more over its lo twin
+  auto encode_pair = [&](CUtensorMap* tm, CUtensorMap* tml, const float* base, const float* lo, int rank, const uint64_t* dims,
+                         const uint64_t* str, const uint32_t* box, const uint32_t* estr) {
+    if (int r = encode_map(tm, base, rank, dims, str, box, estr, f16)) return r;
+    if (!d.split) { *tml = *tm; return 0; }
+    return encode_map(tml, lo, rank, dims, str, box, estr, f16);
+  };
   const int bke = f16 ? 64 : BKE;            // elements per 128-byte K step
   const uint64_t es = f16 ? 2 : 4;           // operand element size
   p.bke = bke;
@@ -704,7 +733,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
       if (!base) continue;
       uint64_t dims[4] = {(uint64_t)C, (uint64_t)Win, (uint64_t)Hin, (uint64_t)d.nimg};
       uint64_t str[3] = {(uint64_t)C * es, (uint64_t)Win * C * es, (uint64_t)Hin * Win * C * es};
-      rc = encode_map(s ? &p.tmA2 : &p.tmA1, base, 4, dims, str, box, estr, f16);
+      rc = encode_pair(s ? &p.tmA2 : &p.tmA1, s ? &p.tmA2l : &p.tmA1l, base, s ? d.a2_lo : d.a1_lo, 4, dims, str, box, estr);
       if (rc) { delete pl; return rc; }
     }
   } else {
@@ -715,13 +744,13 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
       if (!base) continue;
       uint64_t dims[4] = {(uint64_t)(s ? d.C2 : d.C1), (uint64_t)d.a_rows, 1, 1};
       uint64_t str[3] = {(uint64_t)d.a_ld * es, (uint64_t)d.a_ld * es * d.a_rows, (uint64_t)d.a_ld * es * d.a_rows};
-      rc = encode_map(s ? &p.tmA2 : &p.tmA1, base, 4, dims, str, box, nullptr, f16);
+      rc = encode_pair(s ? &p.tmA2 : &p.tmA1, s ? &p.tmA2l : &p.tmA1l, base, s ? d.a2_lo : d.a1_lo, 4, dims, str, box, nullptr);
       if (rc) { delete pl; return rc; }
     }
   }
-  if (!d.a2) p.tmA2 = p.tmA1;
-  p.tmA3 = p.tmA1; p.tmA4 = p.tmA1;
-  p.tmH1 = p.tmA1; p.tmH2 = p.tmA1;
+  if (!d.a2) { p.tmA2 = p.tmA1; p.tmA2l = p.tmA1l; }
+  p.tmA3 = p.tmA1; p.tmA4 = p.tmA1; p.tmA3l = p.tmA1l; p.tmA4l = p.tmA1l;
+  p.tmH1 = p.tmA1; p.tmH2 = p.tmA1; p.tmH1l = p.tmA1l; p.tmH2l = p.tmA1l;
   {
     // Halo form: 'same'-padded stride-1 3x3 filters on 16- or 32-pixel-wide images, where the CTA's tile
     // (256 pixels, swapped form) is whole rows of ONE image: 3 loads of (rows + 2) x W pixels per
@@ -747,7 +776,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
         if (!base) continue;
         uint64_t dims[4] = {(uint64_t)C, (uint64_t)d.W, (uint64_t)d.H, (uint64_t)d.nimg};
         uint64_t str[3] = {(uint64_t)C * es, (uint64_t)d.W * C * es, (uint64_t)d.H * d.W * C * es};
-        rc = encode_map(s ? &p.tmH2 : &p.tmH1, base, 4, dims, str, box, nullptr, f16);
+        rc = encode_pair(s ? &p.tmH2 : &p.tmH1, s ? &p.tmH2l : &p.tmH1l, base, s ? d.a2_lo : d.a1_lo, 4, dims, str, box, nullptr);
         if (rc) { delete pl; return rc; }
       }
     }
@@ -765,7 +794,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
       if (!base) continue;
       uint64_t dims[4] = {(uint64_t)C, (uint64_t)d.W, (uint64_t)d.H, (uint64_t)d.nimg};
       uint64_t str[3] = {(uint64_t)C * es, (uint64_t)d.W * C * es, (uint64_t)d.H * d.W * C * es};
-      rc = encode_map(s ? &p.tmA4 : &p.tmA3, base, 4, dims, str, box, nullptr, f16);
+      rc = encode_pair(s ? &p.tmA4 : &p.tmA3, s ? &p.tmA4l : &p.tmA3l, base, s ? d.a4_lo : d.a3_lo, 4, dims, str, box, nullptr);
       if (rc) { delete pl; return rc; }
     }
     p.kchunks3 = d.C3 / bke; p.kchunks4 = d.a4 ? d.C4 / bke : 0; p.C3 = d.C3;
@@ -774,14 +803,14 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     uint64_t dims[2] = {(uint64_t)d.K_total, (uint64_t)d.w_rows};
     uint64_t str[1] = {(uint64_t)(d.w_ld ? d.w_ld : d.K_total) * es};
     uint32_t box[2] = {(uint32_t)bke, (uint32_t)(p.swap ? 128 : pl->bn)};
-    rc = encode_map(&p.tmW, d.w, 2, dims, str, box, nullptr, f16);
+    rc = encode_pair(&p.tmW, &p.tmWl, d.w, d.w_lo, 2, dims, str, box, nullptr);
     if (rc) { delete pl; return rc; }
-    p.tmW2 = p.tmW;
+    p.tmW2 = p.tmW; p.tmW2l = p.tmWl;
     if (d.a3) {
       const uint64_t K3 = (uint64_t)d.C3 + (d.a4 ? d.C4 : 0);
       uint64_t dims2[2] = {K3, (uint64_t)d.N_total};
       uint64_t str2[1] = {K3 * es};
-      rc = encode_map(&p.tmW2, d.w2, 2, dims2, str2, box, nullptr, f16);
+      rc = encode_pair(&p.tmW2, &p.tmW2l, d.w2, d.w2_lo, 2, dims2, str2, box, nullptr);
       if (rc) { delete pl; return rc; }
     }
   }
@@ -792,6 +821,10 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
 
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 const char* tc_gemm_form(const TcGemmPlan* p) {
+  if (p->prm.nphase == 3) {
+    if (p->prm.swap) return p->prm.halo ? "swap-halo 3xtf32" : "swap 3xtf32";
+    return p->bn == 256 ? "single256 3xtf32" : "single128 3xtf32";
+  }
   if (p->prm.swap) return p->prm.halo ? "swap-halo" : "swap";
   return p->bn == 256 ? "single256" : "single128";
 }

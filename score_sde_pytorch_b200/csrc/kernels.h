@@ -35,8 +35,11 @@ int launch_fill_from_table(const float* table, const int* step, float* dst, int 
 int launch_nhwc_to_nchw(const float* src, float* dst, int B, int HW, int C, cudaStream_t st);
 // y = x in tensor-core operand format `mode` (store_operand4: 1 TF32 grid, 2 fp16); n % 4 == 0, 16-byte aligned pointers
 int launch_store_operand(const float* x, float* y, long long n, int mode, cudaStream_t st);
+// lo (split TF32, round_out 1 only): dst gets hi = rna_tf32(w), lo the same layout of rna_tf32(w - hi)
 int launch_pack_weight(const float* src, float* dst, int taps, int O, int I, long long so, long long si,
-                       long long stp, int round_out, cudaStream_t st, long long dt = 0, long long dO = 0);
+                       long long stp, int round_out, cudaStream_t st, long long dt = 0, long long dO = 0, float* lo = nullptr);
+// split TF32 pair of an fp32 tensor: hi = rna_tf32(x), lo = rna_tf32(x - hi); n % 4 == 0, 16-byte aligned pointers
+int launch_split_tf32(const float* x, float* hi, float* lo, long long n, cudaStream_t st);
 int launch_im2col3x3_nchw(const float* x, float* patches, int B, int C, int Hin, int Win, int H, int W, int stride,
                           int pad, int mode, cudaStream_t st);
 bool attn_small_supported(int T, int C);   // T <= 64 tokens; q / k staged in channel slabs when 2*T*C floats exceed shared memory
@@ -118,6 +121,11 @@ struct TcGemmDesc {
                             // + 8 = accepted, no effect (every launch of a shape with a halo form walks K in that form's order)
   double* qstats;           // optional GroupNorm quad sums [img][N_total/4][2] accumulated by the epilogue (mode 1)
   Epilogue epi;
+  // split TF32 ("3xTF32"): every operand x is the pair hi = rna_tf32(x) (a1..a4, w, w2) and lo = rna_tf32(x - hi) (the
+  // *_lo twins, same shape and pitch), and each K step runs three products into one fp32 accumulator:
+  // lo_A hi_W + hi_A lo_W + hi_A hi_W (small terms first).  TF32 operands only.
+  int split;
+  const float *a1_lo, *a2_lo, *a3_lo, *a4_lo, *w_lo, *w2_lo;
 };
 int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out);
 void tc_gemm_plan_destroy(TcGemmPlan* p);
@@ -143,7 +151,7 @@ int tc_attn_plan_create(const TcAttnDesc& d, TcAttnPlan** out);
 void tc_attn_plan_destroy(TcAttnPlan* p);
 int tc_attn_launch(const TcAttnPlan* p, cudaStream_t st);
 void tc_gemm_set_head(TcGemmPlan* p, float* out_nchw, const float* per_img_div, long long div_stride);   // per-call pointers of the NCHW head
-const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]"
+const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]", + " 3xtf32" for split TF32
 
 // ---- pc_update.cu -----------------------------------------------------------
 struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` elements

@@ -29,7 +29,9 @@ def positional_frequencies(nf):
 class EngineModel(nn.Module):
   """Base of the engine-backed networks.  ``precision``: ``'tf32'`` (wgmma tensor cores on TF32-rounded fp32 operands,
   default), ``'f16'`` (wgmma on fp16 operands: the same 11-bit significand as TF32 with fp32 accumulation and fp32
-  activations between layers) or ``'fp32'`` (strict fp32 on CUDA cores; validation mode)."""
+  activations between layers), ``'tf32x3'`` (split TF32: every operand as a hi + lo pair of TF32 values, three wgmma
+  products per K step into an fp32 accumulator - close to fp32 accuracy at tensor-core rate) or ``'fp32'`` (strict fp32
+  on CUDA cores; validation mode)."""
 
   def _set_engine_options(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,
                           separate_groupnorm=None, pdl=None, halo=None):
@@ -83,9 +85,9 @@ class EngineModel(nn.Module):
     c.conditional = int(bool(m.conditional))
     c.pdl = int(self.pdl)
     c.no_halo = self.halo if (isinstance(self.halo, int) and not isinstance(self.halo, bool)) else int(not self.halo)
-    if self.precision not in ('tf32', 'fp32', 'f16'):
-      raise ValueError(f"precision must be 'tf32', 'fp32' or 'f16', got {self.precision!r}")
-    c.precision = {'tf32': 0, 'fp32': 1, 'f16': 2}[self.precision]
+    if self.precision not in ('tf32', 'fp32', 'f16', 'tf32x3'):
+      raise ValueError(f"precision must be 'tf32', 'fp32', 'f16' or 'tf32x3', got {self.precision!r}")
+    c.precision = {'tf32': 0, 'fp32': 1, 'f16': 2, 'tf32x3': 3}[self.precision]
     c.keep_activations = int(self.keep_activations)
     c.lanes = self.lanes
     c.cuda_core_head = int(self.cuda_core_head)

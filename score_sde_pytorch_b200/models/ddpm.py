@@ -57,7 +57,7 @@ def _resample(c, down):
 @utils.register_model(name='ddpm')
 class DDPM(EngineModel):
   """DDPM model (engine-backed).  Same execution options as ``NCSNpp``: ``precision`` in ``'tf32'`` (default),
-  ``'f16'``, ``'fp32'``; ``keep_activations`` (debug taps), ``lanes``, ``pdl``.  The 256-pixel configs have 512-channel
+  ``'f16'``, ``'tf32x3'`` (split TF32, close to fp32 accuracy on the tensor cores), ``'fp32'``; ``keep_activations`` (debug taps), ``lanes``, ``pdl``.  The 256-pixel configs have 512-channel
   attention at 16x16, which the fused fp16 attention core does not cover: they run in ``'tf32'`` and ``'fp32'``."""
 
   def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,

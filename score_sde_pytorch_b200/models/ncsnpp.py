@@ -112,7 +112,9 @@ class NCSNpp(EngineModel):
   """NCSN++ model (engine-backed).  ``precision``: ``'tf32'`` (wgmma tensor cores on TF32-rounded
   fp32 operands, default), ``'f16'`` (wgmma on fp16 operands: the same 11-bit significand as TF32
   with fp32 accumulation and fp32 activations between layers, half the operand traffic and twice the
-  MMA rate) or ``'fp32'`` (strict fp32 on CUDA cores; validation mode).  The engine plumbing is
+  MMA rate), ``'tf32x3'`` (split TF32: hi + lo TF32 pairs, three wgmma products per K step; close to fp32
+  accuracy on the tensor cores, about 3x the MMA work of ``'tf32'``) or ``'fp32'`` (strict fp32 on CUDA cores;
+  validation mode).  The engine plumbing is
   ``models._engine.EngineModel``."""
 
   def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,
