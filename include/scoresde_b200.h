@@ -130,11 +130,7 @@ typedef struct {
                                  * streams (batches >= 128).  Off by default. */
   int cuda_core_head;           /* 1: the output convolution (ncsnpp.py:374-380) runs on CUDA cores with an fp32 input in
                                  * every precision mode (costs ~1.4 % of a step, buys back ~1e-4 of rel-L2); 0: tensor cores */
-  int separate_groupnorm;       /* 1: every GroupNorm+SiLU of the tensor-core layers is its own streaming pass; the few-channel
-                                 * convolutions of the nf = 16 networks (csrc/conv_lowc.cu, TF32 mode) are memory-bound and apply
-                                 * their GroupNorm+SiLU on load; 2: separate passes there too.  0 (GroupNorm on load by the
-                                 * tensor-core convolution) is not available in this build and is rejected by b200_ncsnpp_create. */
-  int embedding_type;           /* 0: Gaussian Fourier features of log(sigma) (layerspp.py:32-41, all_modules[0].W); 1: sinusoidal
+  int embedding_type;          /* 0: Gaussian Fourier features of log(sigma) (layerspp.py:32-41, all_modules[0].W); 1: sinusoidal
                                  * positional embedding of the time label (layers.py:515-529, ncsnpp.py:242-247): no module,
                                  * the frequency table is the pseudo-parameter "pos_freqs" [nf/2] */
   int naive_resample;           /* 0: FIR up/down-sampling in the resblocks (fir=True); 1: nearest-neighbour 2x upsampling and
@@ -145,18 +141,18 @@ typedef struct {
   int pdl;                      /* 1: every launch of a forward / PC iteration carries the programmatic-dependent-launch attribute
                                  * (each kernel waits for its predecessor with griddepcontrol.wait after its own prologue, so launch
                                  * latency and barrier init of kernel k+1 overlap the tail of kernel k) */
-  int no_halo;                  /* (the Python host sets 2 unless told otherwise.)  0 or 2: swapped-form 3x3 'same' convolutions on
-                                 * 16- / 32-pixel-wide images read three W-shifted halo copies of their tile per channel chunk (csrc/gemm_tc.cu
-                                 * "halo form": 2.4x fewer L2 -> shared-memory bytes than one shifted tile per filter tap); 1: one shifted
-                                 * tile per tap everywhere (kept for A/B); + 4: with an L2 prefetch of the next tile's halo boxes; + 8:
-                                 * accepted and ignored (it used to make row-major launches walk K in the halo form's order, which every
-                                 * launch of such a shape now does).  Results are bit-identical in every mode (same products, same order). */
+  int no_halo;                  /* 0 (default): swapped-form 3x3 'same' convolutions on 16- / 32-pixel-wide images read three
+                                 * W-shifted halo copies of their tile per channel chunk (csrc/gemm_tc.cu "halo form": 2.4x fewer
+                                 * L2 -> shared-memory bytes than one shifted tile per filter tap); 1: one shifted tile per tap
+                                 * everywhere (kept for A/B).  Results are bit-identical in both modes (same products, same order).
+                                 * Other values are rejected by b200_ncsnpp_create. */
   int family;                   /* 0 = NCSN++ / DDPM++ (models/ncsnpp.py, the default); 1 = DDPM (models/ddpm.py:39-181): ResnetBlockDDPM
                                  * with the NIN_0 skip (layers.py:619-662), AttnBlock (:558-581), Downsample / Upsample with_conv
                                  * (:584-616), residual scale 1, GroupNorm with 32 groups everywhere (channel counts must be multiples
                                  * of 32), sinusoidal time embedding through the "pos_freqs" pseudo-parameter.  Family 1 reads
                                  * image_size, num_channels, nf, num_res_blocks, num_levels, ch_mult, num_attn_resolutions,
-                                 * attn_resolutions, centered and the execution fields (precision ... no_halo); it requires
+                                 * attn_resolutions, centered and the execution fields (precision, keep_activations, lanes,
+                                 * cuda_core_head, pdl, no_halo, tangent); it requires
                                  * conditional = 1 and scale_by_sigma = 0, and ignores skip_rescale, progressive_input, progressive,
                                  * fir_taps / fir_kernel, naive_resample and embedding_type. */
   int tangent;                  /* 0 (default): the forward alone.  1: the plan also carries the forward-mode tangent pass of

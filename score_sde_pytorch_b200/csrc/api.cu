@@ -29,7 +29,7 @@ using namespace b200;
 extern "C" {
 
 const char* b200_last_error(void) { return last_error(); }
-int b200_version(void) { return 100; }   // 0.1.0
+int b200_version(void) { return 200; }   // 0.2.0
 
 int b200_device_sm_count(int* out) {
   int dev = 0, n = 0;

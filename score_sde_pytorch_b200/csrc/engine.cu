@@ -468,7 +468,7 @@ struct Builder {
     split = e_->cfg.precision == 3;
     om = e_->cfg.precision == 2 ? 2 : split ? 0 : 1;
     tan = e_->cfg.tangent != 0;
-    lowc_gn = e_->cfg.precision == 0 && e_->cfg.separate_groupnorm != 2 && !tan;
+    lowc_gn = e_->cfg.precision == 0 && !tan;
     if (dry_) stats_base = reinterpret_cast<char*>(uintptr_t(1) << 40);   // any non-null base: only offsets matter in a dry run
   }
   // the tangent of t as a tensor of its own (for the linear ops, which run the forward kernels on it)
@@ -1326,8 +1326,8 @@ extern "C" {
 
 int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
   B200_REQUIRE(cfg && out, "ncsnpp_create: null argument");
-  B200_REQUIRE(cfg->separate_groupnorm != 0, "ncsnpp_create: separate_groupnorm = 0 (GroupNorm applied on load by the tensor-core "
-               "convolution) is not available in this build; use 1 or 2");
+  B200_REQUIRE(cfg->no_halo == 0 || cfg->no_halo == 1, "ncsnpp_create: no_halo=%d unknown (0 halo form, 1 one tile per tap)",
+               cfg->no_halo);
   B200_REQUIRE(cfg->family == 0 || cfg->family == 1, "ncsnpp_create: family=%d unknown (0 NCSN++, 1 DDPM)", cfg->family);
   B200_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, "ncsnpp_create: precision=%d unknown (0 tf32, 1 fp32, 2 f16, 3 split tf32)",
                cfg->precision);

@@ -58,7 +58,6 @@ struct TcParams {
   int halo;                               // 1: 3x3 taps read W-shifted halo copies of the tile (3 loads per channel chunk instead of 9)
   int halo_dh_bytes;                       // W * 128: bytes between the operand windows of consecutive filter rows inside a copy
   int halo_copy_bytes;                     // (tile rows + 2) * W * 128: bytes of one halo copy
-  int halo_prefetch;                       // 1: the halo producers prefetch the next tile's halo boxes (all channel chunks) into L2 (opt-in: measured -2 %)
   int chunk_major;                         // nine-load loop walks K as (chunk, filter column, filter row): shapes with a halo form
   int conv, H, W, taps, pad, S, stride;   // H, W: OUTPUT spatial size; S = filter width (3 or 1)
   int kchunks1, kchunks2, C1;
@@ -116,12 +115,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, void* dst, ui
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
-}
-
-// fire-and-forget: pull a 4-D box towards L2 (UTMAPF); the halo producers use it for the NEXT tile's whole channel vector so
-// that DRAM sees each pixel row once, contiguously, instead of one 128-byte chunk per K phase
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(tm), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -436,12 +429,6 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
         const int p0 = (tile / p.tiles_n) * 256;
         const int img0 = (int)(p0 / HW), h0 = (int)(p0 % HW) / p.W;
         const int wrow0 = nt * 128;
-        if (issue && p.halo_prefetch && tile + gridDim.x < p.total_tiles && (tile + gridDim.x) / p.tiles_n != tile / p.tiles_n) {
-          const int q0 = ((tile + gridDim.x) / p.tiles_n) * 256;                 // next tile of this CTA: its pixels, every chunk
-          const int qi = (int)(q0 / HW), qh = (int)(q0 % HW) / p.W;
-          for (int kc = 0; kc < p.kchunks1; ++kc) tma_prefetch_4d(&p.tmH1, kc * bke, 0, qh - 1, qi);
-          for (int kc = 0; kc < p.kchunks2; ++kc) tma_prefetch_4d(&p.tmH2, kc * bke, 0, qh - 1, qi);
-        }
         for (int src = 0; src < 4; ++src) {
           const int nch = src == 0 ? p.kchunks1 : src == 1 ? p.kchunks2 : src == 2 ? p.kchunks3 : p.kchunks4;
           if (nch == 0) continue;
@@ -756,7 +743,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     // (256 pixels, swapped form) is whole rows of ONE image: 3 loads of (rows + 2) x W pixels per
     // channel chunk instead of 9 loads of rows x W - the plain form is bound by the L2 -> SM fill rate, not the tensor pipe.
     const int tile_px = p.swap ? 256 : BM;
-    const bool halo = (d.no_halo & 3) != 1 && d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && p.swap &&
+    const bool halo = !d.no_halo && d.conv && d.taps == 9 && p.pad == 1 && p.stride == 1 && p.swap &&
                       (d.W == 16 || d.W == 32) && (d.H * d.W) % tile_px == 0 && (d.Hin == 0 || d.Hin == d.H) && (d.Win == 0 || d.Win == d.W);
     // every launch of a shape that has a halo form walks K in that form's order, swapped or row-major, halo on or off: the
     // A/B of the two mainloops is bit-identical, and a row-major launch of such a shape (one the swapped form does not
@@ -767,7 +754,6 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     if (halo) {
       const int rows = tile_px / d.W;
       p.halo = 1; p.halo_dh_bytes = d.W * 128; p.halo_copy_bytes = (rows + 2) * d.W * 128;
-      p.halo_prefetch = (d.no_halo & 4) ? 1 : 0;
       B200_REQUIRE(p.halo_copy_bytes <= HALO_X_BYTES, "gemm_tc: halo copy of %d bytes does not fit its slot", p.halo_copy_bytes);
       uint32_t box[4] = {(uint32_t)bke, (uint32_t)d.W, (uint32_t)(rows + 2), 1};
       for (int s = 0; s < 2; ++s) {

@@ -116,9 +116,7 @@ struct TcGemmDesc {
   const float* a3; int C3; const float* a4; int C4; const float* w2;
   int f16;                  // 1: a1..a4, w, w2 hold fp16 elements (wgmma .f16, 64-channel K steps); pitches stay in elements
   int no_halo;              // halo form of the 3x3 mainloop (three W-shifted halo copies per channel chunk instead of nine shifted
-                            // tiles): 0 or 2 = in the swapped form, 1 = never;
-                            // + 4 = with an L2 prefetch (UTMAPF) of the next tile's halo boxes (A/B: measured 2 % slower);
-                            // + 8 = accepted, no effect (every launch of a shape with a halo form walks K in that form's order)
+                            // tiles): 0 = in the swapped form, 1 = never (same K order either way)
   double* qstats;           // optional GroupNorm quad sums [img][N_total/4][2] accumulated by the epilogue (mode 1)
   Epilogue epi;
   // split TF32 ("3xTF32"): every operand x is the pair hi = rna_tf32(x) (a1..a4, w, w2) and lo = rna_tf32(x - hi) (the

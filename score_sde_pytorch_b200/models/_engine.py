@@ -33,29 +33,19 @@ class EngineModel(nn.Module):
   products per K step into an fp32 accumulator - close to fp32 accuracy at tensor-core rate) or ``'fp32'`` (strict fp32
   on CUDA cores; validation mode)."""
 
-  def _set_engine_options(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,
-                          separate_groupnorm=None, pdl=None, halo=None):
+  def _set_engine_options(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None, pdl=None,
+                          halo=None):
     m = config.model
     self.precision = (precision or getattr(m, 'precision', 'tf32')).lower()
     self.keep_activations = bool(keep_activations)
     self.lanes = int(getattr(m, 'lanes', lanes))   # 2: evaluate batches >= 128 as two half-batch lanes on two streams
     # per-engine execution options (fields of b200_ncsnpp_config; nothing is read from the environment)
     self.cuda_core_head = bool(getattr(m, 'cuda_core_head', False) if cuda_core_head is None else cuda_core_head)
-    # GroupNorm+SiLU of the tensor-core layers runs as a stand-alone streaming pass (True, default).  The convolution that
-    # applied it on load (False) is not part of this build, so False is rejected rather than silently ignored.
-    # (2: separate passes also in front of the memory-bound few-channel convolutions of the nf = 16 networks, which
-    # otherwise normalise on load in tf32 mode - csrc/conv_lowc.cu; kept for A/B tests)
-    sg = getattr(m, 'separate_groupnorm', True) if separate_groupnorm is None else separate_groupnorm
-    if not sg:
-      raise ValueError(f'{type(self).__name__}: separate_groupnorm=False (GroupNorm applied on load by the tensor-core '
-                       'convolution) is not available in this build; use True (separate pass) or 2')
-    self.separate_groupnorm = 2 if (not isinstance(sg, bool) and sg == 2) else True
     # programmatic dependent launch between the kernels of a forward / PC iteration (common.cuh)
     self.pdl = bool(getattr(m, 'pdl', PDL_DEFAULT) if pdl is None else pdl)
     # halo form of the 3x3 tensor-core mainloop (csrc/gemm_tc.cu): True (default) = in the swapped-operand kernel, False =
-    # nine shifted tile loads per channel chunk (kept for A/B); an int is the raw b200_ncsnpp_config.no_halo (tests: 8)
-    hv = getattr(m, 'halo', HALO_DEFAULT) if halo is None else halo
-    self.halo = hv if (isinstance(hv, int) and not isinstance(hv, bool)) else bool(hv)   # int: raw b200_ncsnpp_config.no_halo
+    # nine shifted tile loads per channel chunk (kept for A/B; bit-identical results)
+    self.halo = bool(getattr(m, 'halo', HALO_DEFAULT) if halo is None else halo)
 
   def _init_engine(self):
     """Call once ``all_modules`` is complete."""
@@ -84,14 +74,13 @@ class EngineModel(nn.Module):
     c.centered, c.scale_by_sigma = int(bool(cfg.data.centered)), int(bool(m.scale_by_sigma))
     c.conditional = int(bool(m.conditional))
     c.pdl = int(self.pdl)
-    c.no_halo = self.halo if (isinstance(self.halo, int) and not isinstance(self.halo, bool)) else int(not self.halo)
+    c.no_halo = int(not self.halo)
     if self.precision not in ('tf32', 'fp32', 'f16', 'tf32x3'):
       raise ValueError(f"precision must be 'tf32', 'fp32', 'f16' or 'tf32x3', got {self.precision!r}")
     c.precision = {'tf32': 0, 'fp32': 1, 'f16': 2, 'tf32x3': 3}[self.precision]
     c.keep_activations = int(self.keep_activations)
     c.lanes = self.lanes
     c.cuda_core_head = int(self.cuda_core_head)
-    c.separate_groupnorm = int(self.separate_groupnorm)
     self._family_config(c)
     return c
 
@@ -295,7 +284,7 @@ class EngineModel(nn.Module):
     inputs of the skip projections - as IEEE fp16, which assumes |value| < 65504 (and loses precision below 6e-5);
     random-init and normalised activations are far inside, a trained checkpoint can be checked with this before it is
     sampled in fp16 mode.  Returns ``{'max_abs': {module_index: float}, 'worst': (index, value), 'fits_f16': bool}``."""
-    probe = type(self)(self.config, precision='tf32', keep_activations=True, separate_groupnorm=True, pdl=False).to(x.device)
+    probe = type(self)(self.config, precision='tf32', keep_activations=True, pdl=False).to(x.device)
     probe.load_state_dict(self.state_dict())
     with torch.no_grad():
       probe(x, time_cond)

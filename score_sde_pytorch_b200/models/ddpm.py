@@ -60,8 +60,8 @@ class DDPM(EngineModel):
   ``'f16'``, ``'tf32x3'`` (split TF32, close to fp32 accuracy on the tensor cores), ``'fp32'``; ``keep_activations`` (debug taps), ``lanes``, ``pdl``.  The 256-pixel configs have 512-channel
   attention at 16x16, which the fused fp16 attention core does not cover: they run in ``'tf32'`` and ``'fp32'``."""
 
-  def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,
-               separate_groupnorm=None, pdl=None, halo=None):
+  def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None, pdl=None,
+               halo=None):
     super().__init__()
     self.config = config
     m = config.model
@@ -75,7 +75,7 @@ class DDPM(EngineModel):
     if m.nonlinearity.lower() != 'swish':
       raise NotImplementedError('DDPM: engine implements the swish (SiLU) nonlinearity only')
     self.register_buffer('sigmas', torch.tensor(utils.get_sigmas(config)))   # fp64, as ddpm.py:44
-    self._set_engine_options(config, precision, keep_activations, lanes, cuda_core_head, separate_groupnorm, pdl, halo)
+    self._set_engine_options(config, precision, keep_activations, lanes, cuda_core_head, pdl, halo)
     nf, ch_mult, nrb = m.nf, tuple(m.ch_mult), m.num_res_blocks
     if nf % 2 or nf < 4:
       raise NotImplementedError('DDPM: the sinusoidal time embedding needs an even nf >= 4')

@@ -117,8 +117,8 @@ class NCSNpp(EngineModel):
   validation mode).  The engine plumbing is
   ``models._engine.EngineModel``."""
 
-  def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None,
-               separate_groupnorm=None, pdl=None, halo=None):
+  def __init__(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None, pdl=None,
+               halo=None):
     super().__init__()
     self.config = config
     m = config.model
@@ -135,7 +135,7 @@ class NCSNpp(EngineModel):
     assert emb != 'fourier' or config.training.continuous, "Fourier features are only used for continuous training."
     self.register_buffer('sigmas', torch.tensor(utils.get_sigmas(config)))   # fp64, as ncsnpp.py:42
     self.embedding_type = emb
-    self._set_engine_options(config, precision, keep_activations, lanes, cuda_core_head, separate_groupnorm, pdl, halo)
+    self._set_engine_options(config, precision, keep_activations, lanes, cuda_core_head, pdl, halo)
     nf, ch_mult, nrb = m.nf, tuple(m.ch_mult), m.num_res_blocks
     L = len(ch_mult)
     all_res = [config.data.image_size // (2 ** i) for i in range(L)]

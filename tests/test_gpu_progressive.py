@@ -61,31 +61,26 @@ def test_progressive_nofir_matches_oracle(dev):
     assert rel_l2(model(x, sigma), NO.ncsnpp_forward(sd, cfg, x, sigma)) < 1e-4
 
 
-def test_few_channel_levels_groupnorm_on_load_matches_separate_passes(dev):
+def test_few_channel_levels_groupnorm_on_load_matches_oracle(dev):
   """nf = 16 network in tf32 mode: the 16/32-channel 3x3 convolutions run on conv_lowc.cu and apply GroupNorm+SiLU while
-  they stage their input (default); separate_groupnorm=2 keeps a streaming GroupNorm pass in front of them.  The two plans
-  differ only by the SiLU flavour (ex2/rcp approximations vs expf/divide, both followed by the TF32 rounding), i.e. by
-  rare one-ulp flips of 11-bit operands: each is held against the oracle, and against each other."""
+  they stage their input.  Held against the oracle at 7.5e-4: the same network with a separate GroupNorm pass in front of
+  those convolutions measured 5.3e-4 on these inputs (H100), and the two plans differ only by rare one-ulp flips of 11-bit
+  operands (ex2/rcp SiLU approximations vs expf/divide, both followed by the TF32 rounding)."""
   from score_sde_pytorch_b200 import configs
   cfg = configs.tiny_progressive(nf=16, image_size=64, num_res_blocks=2, ch_mult=(1, 2, 2, 4), attn_resolutions=(8,))
   torch.manual_seed(3)
-  fused = seeded_model(cfg, precision='tf32').to(dev)
-  separate = seeded_model(cfg, precision='tf32', separate_groupnorm=2).to(dev)
-  separate.load_state_dict(fused.state_dict())
-  sd = {k: v.to(dev) for k, v in fused.state_dict().items()}
+  model = seeded_model(cfg, precision='tf32').to(dev)
+  sd = {k: v.to(dev) for k, v in model.state_dict().items()}
   torch.manual_seed(5)
   x = torch.randn(3, 3, 64, 64, device=dev) * 3
   sigma = torch.tensor([20.0, 1.5, 0.05], device=dev)
   with torch.no_grad():
-    yf, ys = fused(x, sigma), separate(x, sigma)
+    y = model(x, sigma)
     ref = NO.ncsnpp_forward(sd, cfg, x, sigma)
-  ef, es, ab = rel_l2(yf, ref), rel_l2(ys, ref), rel_l2(yf, ys)
-  nf_, ns_ = fused.launches_per_forward(), separate.launches_per_forward()
-  print(f'few-channel GroupNorm on load: vs oracle {ef:.3e} (separate passes {es:.3e}), fused vs separate {ab:.3e}; launches {nf_} vs {ns_}')
-  assert nf_ <= ns_
-  assert any('gn+silu' in n for n in fused.op_names()) and not any('gn+silu' in n for n in separate.op_names())
-  assert es < 1e-3 and ef < 1.25 * es + 1e-4
-  assert ab < 1e-3
+  e = rel_l2(y, ref)
+  print(f'few-channel GroupNorm on load: vs oracle {e:.3e}; {model.launches_per_forward()} launches')
+  assert any('gn+silu' in n for n in model.op_names())
+  assert e < 7.5e-4
 
 
 @pytest.mark.parametrize('name,precision', [('celebahq_256', 'tf32'), ('celebahq_256', 'f16'), ('ffhq_1024', 'tf32')])

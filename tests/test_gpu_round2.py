@@ -146,9 +146,7 @@ def test_forward_batch256_plan_matches_small_batch_plan_and_oracle(dev, precisio
   SAMPLER output and is held by test_pc_sampler_cifar10_full_1000_steps_within_parity_bound and by bench.py's in-run
   check at batch 1024, so (b) only guards against gross errors."""
   cfg = golden_config('cifar10_ve')
-  # no_halo = 2 | 8: the default plan plus "row-major launches of shapes with a halo form walk K in that form's order", so
-  # that the batch-256 and batch-8 plans add the products in the same order
-  model = seeded_model(cfg, precision=precision, halo=2 | 8).to(dev)
+  model = seeded_model(cfg, precision=precision).to(dev)
   sd = {k: v.to(dev) for k, v in model.state_dict().items()}
   B = 256
   torch.manual_seed(9)
@@ -158,6 +156,7 @@ def test_forward_batch256_plan_matches_small_batch_plan_and_oracle(dev, precisio
     ref = _oracle_net(cfg, sd)(x, sigma)
     y = model(x, sigma).clone()
     y2 = model(x, sigma).clone()
+    assert any('[swap-halo]' in n for n in model.op_names())   # the batch-256 plan
     ys = torch.cat([model(x[i:i + 8], sigma[i:i + 8]).clone() for i in range(0, 64, 8)])
   small = ((y[:64] - ys).flatten(1).double().norm(dim=1) / ys.flatten(1).double().norm(dim=1))
   per_img = ((y - ref).flatten(1).double().norm(dim=1) / ref.flatten(1).double().norm(dim=1))
@@ -171,19 +170,6 @@ def test_forward_batch256_plan_matches_small_batch_plan_and_oracle(dev, precisio
   s1 = torch.full((B,), 3.3, device=dev)
   with torch.no_grad():
     assert rel_l2(model(x, s1, labels_uniform=True), model(x, s1)) < 2e-5
-  # and the package default: the same launches; its row-major convolutions walk K tap-major instead of chunk-major, so it
-  # re-rolls the 11-bit operand roundings and is held to the oracle with the same bounds, not to the other plan
-  # its own batch-8 plans add the products in the same (tap-major) order, so (a) holds for it as tightly
-  dflt = seeded_model(cfg, precision=precision).to(dev)
-  with torch.no_grad():
-    yd = dflt(x, sigma).clone()
-  assert dflt.op_names() == model.op_names() and any('[swap-halo]' in n for n in dflt.op_names())   # both batch-256 plans
-  with torch.no_grad():
-    yds = torch.cat([dflt(x[i:i + 8], sigma[i:i + 8]).clone() for i in range(0, 64, 8)])
-  small_d = ((yd[:64] - yds).flatten(1).double().norm(dim=1) / yds.flatten(1).double().norm(dim=1))
-  assert small_d.max().item() < 5e-5
-  per_img_d = ((yd - ref).flatten(1).double().norm(dim=1) / ref.flatten(1).double().norm(dim=1))
-  assert per_img_d.max().item() < 3e-3 and per_img_d.median().item() < 1.5e-3
 
 
 @pytest.mark.parametrize('case', ['tiny_fp32', 'cifar10_f16'])

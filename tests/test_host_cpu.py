@@ -207,7 +207,7 @@ def test_affine_tables_reproduce_ancestral_sampling_and_annealed_langevin():
 
 def test_library_loads_and_exports_every_declared_symbol():
   lib = _lib.load()
-  assert lib.b200_version() >= 100
+  assert lib.b200_version() >= 200   # the b200_ncsnpp_config layout of _lib.NcsnppConfig
   header = open(os.path.join(REPO, 'include', 'scoresde_b200.h')).read()
   declared = set(re.findall(r'B200_API\s+[\w\s\*]+?\b(b200_\w+)\s*\(', header))
   assert declared, 'no declarations parsed'
@@ -384,15 +384,17 @@ def test_parameter_list_matches_the_reference_order(name):
 
 def test_execution_options_reach_the_native_config():
   """Per-engine options are fields of b200_ncsnpp_config (nothing is read from the environment).  `halo`: the package
-  default is no_halo = 0 (halo form in the swapped kernel); True / False / raw ints map as documented
-  in include/scoresde_b200.h."""
+  default is no_halo = 0 (halo form in the swapped kernel), False gives 1 (one shifted tile per tap); b200_ncsnpp_create
+  rejects any other no_halo."""
   from score_sde_pytorch_b200.models.ncsnpp import NCSNpp
   cfg = golden_config('tiny')
-  want = {None: 0, True: 0, False: 1, 8: 8, 2 | 8: 10, 6: 6}
+  want = {None: 0, True: 0, False: 1}
   for halo, no_halo in want.items():
     m = NCSNpp(cfg) if halo is None else NCSNpp(cfg, halo=halo)
     assert m._native_config().no_halo == no_halo, (halo, m._native_config().no_halo)
-  c = NCSNpp(cfg, precision='f16', separate_groupnorm=2, pdl=True, cuda_core_head=True)._native_config()
-  assert (c.precision, c.separate_groupnorm, c.pdl, c.cuda_core_head) == (2, 2, 1, 1)
-  with pytest.raises(ValueError):           # GroupNorm on load by the tensor-core convolution is not in this build
-    NCSNpp(cfg, precision='f16', separate_groupnorm=False)
+  c = NCSNpp(cfg, precision='f16', pdl=True, cuda_core_head=True)._native_config()
+  assert (c.precision, c.pdl, c.cuda_core_head) == (2, 1, 1)
+  c.no_halo = 4
+  h = ctypes.c_void_p()
+  with pytest.raises(RuntimeError, match='no_halo'):
+    _lib.call('b200_ncsnpp_create', ctypes.byref(c), ctypes.byref(h))

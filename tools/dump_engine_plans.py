@@ -7,8 +7,8 @@ few PC samplers, the launches per step and the PC workspace size.
 tests/test_gpu_engine_plans.py rebuilds the matrix on a GPU and requires the plans to equal the golden exactly;
 tests/test_engine_plans_cpu.py checks the parts that are planned without a device (parameter tables, weight and
 workspace sizes).  The matrix reaches every op the plan builder can emit: each precision, the lane split, both halo
-forms, both heads, the tangent plans, the few-channel kernel with and without GroupNorm on load, and the input_skip /
-output_skip pyramids of the high-resolution networks."""
+forms, both heads, the tangent plans, the few-channel levels with GroupNorm on load (tf32) and behind a separate
+GroupNorm pass (tf32x3), and the input_skip / output_skip pyramids of the high-resolution networks."""
 import argparse
 import ctypes
 import gzip
@@ -32,7 +32,7 @@ WS_BATCHES = (1, 8, 256)   # workspace sizes are recorded at these batches and a
 
 def _config(name):
   if name == 'nf16_progressive':
-    # the nf = 16 few-channel network of test_few_channel_levels_groupnorm_on_load_matches_separate_passes
+    # the nf = 16 few-channel network of test_few_channel_levels_groupnorm_on_load_matches_oracle
     return configs.tiny_progressive(nf=16, image_size=64, num_res_blocks=2, ch_mult=(1, 2, 2, 4), attn_resolutions=(8,))
   if name == 'tiny_ddpm':
     return configs.tiny_ddpm()
@@ -60,7 +60,7 @@ def cases():
     if name in ('tiny_ddpm', 'tiny_ddpmpp'):
       out += [_case(name, p, tangent=True) for p in ('fp32', 'tf32')]
   out.append(_case('tiny', 'tf32', keep_activations=True))
-  out += [_case('nf16_progressive', 'tf32', separate_groupnorm=sg) for sg in (True, 2)]
+  out += [_case('nf16_progressive', p) for p in ('tf32', 'tf32x3')]
   out += [_case(name, 'tf32', batch=1) for name in ('celebahq_256', 'ffhq_1024')]
   return out
 

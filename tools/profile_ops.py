@@ -19,8 +19,7 @@ ap.add_argument('--precision', default='f16')
 ap.add_argument('--reps', type=int, default=5)
 ap.add_argument('--md', default=None)
 ap.add_argument('--config', default='headline', choices=['headline', 'celebahq_256', 'ddpmpp_256', 'ffhq_1024', 'cifar10_ddpmpp'])
-ap.add_argument('--no-halo', action='store_true', help='round-1 3x3 mainloop: one shifted tile load per filter tap')
-ap.add_argument('--halo-mode', type=int, default=None, help='raw b200_ncsnpp_config.no_halo (0 swap only, 1 off, 2 pairs too, +4 with L2 prefetch of the next tile)')
+ap.add_argument('--no-halo', action='store_true', help='3x3 mainloop with one shifted tile load per filter tap everywhere')
 args = ap.parse_args()
 dev = torch.device('cuda:0')
 torch.manual_seed(0)
@@ -29,7 +28,7 @@ cfg = {'headline': headline_config, 'celebahq_256': configs.ve_celebahq_256_ncsn
        'ddpmpp_256': configs.subvp_celebahq_256_ddpmpp_continuous, 'ffhq_1024': configs.ve_ffhq_1024_ncsnpp_continuous,
        'cifar10_ddpmpp': configs.vp_cifar10_ddpmpp_continuous}[args.config]()
 cfg.model.init_scale = 1.0
-model = NCSNpp(cfg, precision=args.precision, halo=(args.halo_mode if args.halo_mode is not None else False if args.no_halo else None)).to(dev)
+model = NCSNpp(cfg, precision=args.precision, halo=not args.no_halo).to(dev)
 B = args.batch
 eng = model.engine(B, dev)
 h = eng['h']
