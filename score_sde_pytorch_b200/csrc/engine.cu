@@ -12,9 +12,6 @@
 #include <string>
 #include <vector>
 
-namespace b200 {
-void tc_gemm_set_rowvec_ld(TcGemmPlan* p, long long ld);
-}
 using namespace b200;
 
 namespace {

@@ -2,6 +2,7 @@
 // and the kernel translation units.  Every launcher returns 0 on success and has
 // already recorded the message for b200_last_error() otherwise.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <algorithm>
@@ -93,6 +94,10 @@ bool conv_lowc_supported(const SimtConv& p);
 int launch_conv_lowc(const SimtConv& p, cudaStream_t st);
 
 // ---- gemm_tc.cu : wgmma / TMA implicit GEMM (TF32 or fp16 operands) --------
+// TMA tensor map (SWIZZLE_128B, zero out-of-bounds fill) over fp32 or fp16 elements; also used by attn_tc.cu
+int encode_map(CUtensorMap* tm, const float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+               const uint32_t* box, const uint32_t* elem_strides = nullptr, bool f16 = false);
+int num_sms();   // of the current device
 struct TcGemmPlan;   // opaque, owns the encoded tensor maps
 struct TcGemmDesc {
   // A: NHWC activations, values already on the TF32 grid.
@@ -129,7 +134,11 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out);
 void tc_gemm_plan_destroy(TcGemmPlan* p);
 int tc_gemm_launch(const TcGemmPlan* p, cudaStream_t st);
 bool tc_gemm_supported(const TcGemmDesc& d, const char** why);
-// fused attention core (logits, softmax, P.V, NIN_3, residual, rescale, quad sums) for T=256 tokens x C=256 channels
+void tc_gemm_set_head(TcGemmPlan* p, float* out_nchw, const float* per_img_div, long long div_stride);   // per-call pointers of the NCHW head
+void tc_gemm_set_rowvec_ld(TcGemmPlan* p, long long ld);   // epi.rowvec_ld of a built plan
+const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]", + " 3xtf32" for split TF32
+
+// ---- attn_tc.cu : fused attention core (logits, softmax, P.V, NIN_3, residual, rescale, quad sums), T=256 x C=256 --
 struct TcAttnPlan;
 struct TcAttnDesc {
   const float* qk;          // [nimg*T][2C]: q | k rows (TF32 grid)
@@ -148,8 +157,6 @@ bool tc_attn_supported(int T, int C);
 int tc_attn_plan_create(const TcAttnDesc& d, TcAttnPlan** out);
 void tc_attn_plan_destroy(TcAttnPlan* p);
 int tc_attn_launch(const TcAttnPlan* p, cudaStream_t st);
-void tc_gemm_set_head(TcGemmPlan* p, float* out_nchw, const float* per_img_div, long long div_stride);   // per-call pointers of the NCHW head
-const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]", + " 3xtf32" for split TF32
 
 // ---- pc_update.cu -----------------------------------------------------------
 struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` elements

@@ -60,7 +60,7 @@ def conv_skip_nhwc(x, s1, s2, wp, bias, wskip, bias_skip, cout, residual=None, s
 
 def attention_core(qk, vT, w3, bv, b3, x, out_scale, want_stats=False):
   """qk [nimg*T, 2C], vT [nimg, C, T], w3 [C, C] (out, in), x [nimg*T, C] -> out [nimg*T, C] (+ quad sums).
-  fp16 qk/vT/w3 select the kind::f16 variant."""
+  fp16 qk/vT/w3 select the wgmma .f16 variant."""
   nimg, C, T = vT.shape
   f16 = qk.dtype == torch.float16
   assert vT.dtype == qk.dtype and w3.dtype == qk.dtype

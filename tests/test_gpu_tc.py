@@ -44,7 +44,7 @@ CASES = [
 
 
 @pytest.mark.parametrize('case', CASES, ids=lambda c: 'B{B}_{H}x{W}_{C1}+{C2}->{Cout}_k{k}'.format(**c))
-def test_tcgen05_conv_matches_cuda_core_conv(dev, case):
+def test_wgmma_conv_matches_cuda_core_conv(dev, case):
   import gpu_util
   B, H, W, C1, C2, Cout, k = (case[x] for x in ('B', 'H', 'W', 'C1', 'C2', 'Cout', 'k'))
   torch.manual_seed(6)
@@ -136,8 +136,8 @@ F16_CASES = [c for c in CASES if c['C1'] % 64 == 0 and c['C2'] % 64 == 0]
 
 
 @pytest.mark.parametrize('case', F16_CASES, ids=lambda c: 'B{B}_{H}x{W}_{C1}+{C2}->{Cout}_k{k}'.format(**c))
-def test_tcgen05_f16_conv_matches_torch(dev, case):
-  """kind::f16 form of the same contraction: activations and packed weights are IEEE fp16 in memory (64-channel
+def test_wgmma_f16_conv_matches_torch(dev, case):
+  """wgmma .f16 form of the same contraction: activations and packed weights are IEEE fp16 in memory (64-channel
   K steps), accumulation and epilogue are fp32.  fp16 x fp16 products are exact in fp32, so against torch's fp32
   convolution of the SAME fp16-representable values only the summation order differs."""
   import gpu_util
@@ -201,7 +201,7 @@ SKIP_CASES = [
 
 
 @pytest.mark.parametrize('case', SKIP_CASES, ids=lambda c: 'B{B}_{H}x{W}_{C}|{S1}+{S2}->{Cout}'.format(**c))
-def test_tcgen05_conv_with_fused_skip_projection(dev, case):
+def test_wgmma_conv_with_fused_skip_projection(dev, case):
   """Resblock tail (layerspp.py:268-274): (Conv_1(h) + Conv_2(x)) / sqrt(2) as ONE contraction whose K loop
   appends the 1x1 projection of the (two-source) block input to the nine taps of the 3x3 filter."""
   import gpu_util
@@ -268,7 +268,7 @@ def test_fused_attention_core_matches_torch(dev, nimg):
 
 @pytest.mark.parametrize('nimg', [2, 150])
 def test_fused_attention_core_f16_matches_torch(dev, nimg):
-  """The kind::f16 variant (fp16 q|k, v^T, W3 in memory; E and O' staged as fp16; 3-stage ring)."""
+  """The wgmma .f16 variant (fp16 q|k, v^T, W3 in memory; E and O' staged as fp16; 3-stage ring)."""
   import gpu_util
   torch.manual_seed(31 + nimg)
   T = C = 256
@@ -292,7 +292,7 @@ def test_fused_attention_core_f16_matches_torch(dev, nimg):
   assert torch.allclose(qs[..., 0], o4.sum((1, 3)), rtol=1e-5, atol=1e-3)
 
 
-def test_tcgen05_batched_gemm_attention_shapes(dev):
+def test_wgmma_batched_gemm_attention_shapes(dev):
   import gpu_util
   rt = gpu_util.round_tf32
   torch.manual_seed(7)
