@@ -84,7 +84,8 @@ B200_API int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int
                                      float scale, int round_tf32, float* out, void* stream);
 B200_API int b200_pack_conv_weight_f32(const float* w_oihw, float* w_packed, int c_out, int c_in, int ksize,
                                        int round_tf32, void* stream);
-/* Fused attention core of AttnBlockpp (layerspp.py:82-91) for T=256 tokens x C=256 channels per image:
+/* Fused attention core of AttnBlockpp (layerspp.py:82-91) for T=256 tokens x C=256 channels per image, or T=256 x
+ * C=512 with fp16 operands (a TF32 C=512 core is not implemented and returns an error naming shape and format):
  * out = (softmax(q k^T / sqrt(C)) v + b_v) W3^T + b_3 + x) * out_scale, tensor cores only.
  * qk = [nimg*T][2C] (q | k), vT = [nimg][C][T] (v transposed, without b_v), w3 = [C_out][C_in]; TF32-representable
  * fp32 (operand_f16 = 0) or IEEE fp16 elements (operand_f16 = 1).

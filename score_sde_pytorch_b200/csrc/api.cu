@@ -146,7 +146,9 @@ int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int cs1, con
 int b200_attention_core_f32(const float* qk, const float* vT, const float* w3, const float* bv, const float* b3,
                             const float* x, float* out, double* qstats, int nimg, int t, int c, float out_scale,
                             int operand_f16, void* stream) {
-  B200_REQUIRE(tc_attn_supported(t, c), "attention_core: only T=256, C=256 is implemented (got T=%d C=%d)", t, c);
+  B200_REQUIRE(tc_attn_supported(t, c, operand_f16 != 0),
+               "attention_core: implemented for T=256 with C=256 (tf32 or fp16 operands) or C=512 (fp16 operands only); "
+               "got T=%d C=%d with %s operands", t, c, operand_f16 ? "fp16" : "tf32");
   TcAttnDesc d; memset(&d, 0, sizeof(d));
   d.qk = qk; d.vT = vT; d.w3 = w3; d.bv = bv; d.b3 = b3; d.x = x; d.out = out; d.qstats = qstats;
   d.nimg = nimg; d.T = t; d.C = c; d.out_scale = out_scale; d.f16 = operand_f16 ? 1 : 0;

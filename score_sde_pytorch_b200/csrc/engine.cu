@@ -295,7 +295,7 @@ int build_graph(b200_ncsnpp* e) {
     const int T = res * res;
     m.tcattn = tcmode && (C % 128 == 0) && (T % 128 == 0) && (T <= 1024);
     // fp16 operands: the logits/probabilities never leave the chip, so only the fused core is implemented
-    if (om == 2 && !tc_attn_supported(T, C)) m.tcattn = false;
+    if (om == 2 && !tc_attn_supported(T, C, true)) m.tcattn = false;
     // few tokens (T <= 64: the 4x4 block of CIFAR-10, the 8x8, 512-channel bottleneck of FFHQ-1024): one CTA per image
     // (attn_small_kernel); otherwise the block runs as separate contractions
     const bool small_ok = attn_small_supported(T, C);
@@ -915,10 +915,10 @@ struct Builder {
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
       // [T,T] logits/probabilities and the attention output stay on chip; other token counts (tf32 mode) use separate launches.
-      if (om == 2 && !(tc && m.tc2 && tc_attn_supported(T, C))) {
+      if (om == 2 && !(tc && m.tc2 && tc_attn_supported(T, C, true))) {
         set_error("ncsnpp: fp16 operand mode needs the fused attention core (T=%d C=%d)", T, C); rc = 2; return Tensor();
       }
-      if (tc && m.tc2 && tc_attn_supported(T, C) && !tan && !split) {
+      if (tc && m.tc2 && tc_attn_supported(T, C, om == 2) && !tan && !split) {
         Tensor out = talloc(C, x.H, x.W);
         if (fused_stats) out.qs = qalloc(C);
         if (!dry) {

@@ -139,6 +139,7 @@ void tc_gemm_set_rowvec_ld(TcGemmPlan* p, long long ld);   // epi.rowvec_ld of a
 const char* tc_gemm_form(const TcGemmPlan* p);   // "single256" | "single128" | "swap[-halo]", + " 3xtf32" for split TF32
 
 // ---- attn_tc.cu : fused attention core (logits, softmax, P.V, NIN_3, residual, rescale, quad sums), T=256 x C=256 --
+// (TF32 or fp16 operands) and T=256 x C=512 (fp16 operands)
 struct TcAttnPlan;
 struct TcAttnDesc {
   const float* qk;          // [nimg*T][2C]: q | k rows (TF32 grid)
@@ -153,7 +154,7 @@ struct TcAttnDesc {
   float out_scale;
   int f16;                  // 1: qk, vT, w3 hold fp16 elements
 };
-bool tc_attn_supported(int T, int C);
+bool tc_attn_supported(int T, int C, bool f16);
 int tc_attn_plan_create(const TcAttnDesc& d, TcAttnPlan** out);
 void tc_attn_plan_destroy(TcAttnPlan* p);
 int tc_attn_launch(const TcAttnPlan* p, cudaStream_t st);
