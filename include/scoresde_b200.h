@@ -93,6 +93,13 @@ B200_API int b200_pack_conv_weight_f32(const float* w_oihw, float* w_packed, int
 B200_API int b200_attention_core_f32(const float* qk, const float* vT, const float* w3, const float* bv,
                                      const float* b3, const float* x, float* out, double* qstats, int nimg,
                                      int t, int c, float out_scale, int operand_f16, void* stream);
+/* Flash-style fp16 attention core of AttnBlockpp (layerspp.py:82-86) for T tokens (a multiple of 128, 128 <= T <= 4096)
+ * x C in {128, 256, 512} channels per image: out = softmax(q k^T / sqrt(C)) v + b_v, with an online softmax (the
+ * [T][T] logits never reach memory), tensor cores only.  qk = [nimg*T][2C] (q | k), vT = [nimg][C][T] (v transposed,
+ * without b_v), out = [nimg*T][C]: IEEE fp16 elements; bv = [C] fp32.  Other shapes, null pointers and nimg < 1
+ * return an error naming the shape.  Deterministic: no atomics. */
+B200_API int b200_attention_flash_f16(const void* qk, const void* vT, const float* bv, void* out, int nimg, int t,
+                                      int c, void* stream);
 /* batched C[b] = A[b] (M x K, pitch lda) * W[b]^T (N x K, pitch ldw), row-major out pitch ldo. */
 B200_API int b200_gemm_nt_f32(const float* a, long long lda, int a_batch_rows, const float* w, long long ldw,
                               int w_batch_rows, int nbatch, int m, int n, int k, const float* bias,

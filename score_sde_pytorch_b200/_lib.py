@@ -63,6 +63,7 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_float, c_int, c_void_p, c_void_p]),
   'b200_attention_core_f32': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int, c_int, c_int, c_float, c_int, c_void_p]),
+  'b200_attention_flash_f16': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
   'b200_pack_conv_weight_f32': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
   'b200_gemm_nt_f32': (c_int, [c_void_p, c_ll, c_int, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_int, c_void_p, c_ll, c_int, c_void_p]),

@@ -159,6 +159,13 @@ int b200_attention_core_f32(const float* qk, const float* vT, const float* w3, c
   return r;
 }
 
+int b200_attention_flash_f16(const void* qk, const void* vT, const float* bv, void* out, int nimg, int t, int c,
+                              void* stream) {
+  AttnFlashPlan pl;
+  if (int r = attn_flash_plan(qk, vT, bv, out, nimg, t, c, &pl)) return r;
+  return attn_flash_launch(pl, static_cast<cudaStream_t>(stream));
+}
+
 int b200_gemm_nt_f32(const float* a, long long lda, int a_batch_rows, const float* w, long long ldw, int w_batch_rows,
                      int nbatch, int m, int n, int k, const float* bias, int round_tf32, float* out, long long ldo,
                      int impl, void* stream) {

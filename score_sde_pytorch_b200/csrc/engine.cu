@@ -294,8 +294,9 @@ int build_graph(b200_ncsnpp* e) {
     Mod m; m.kind = M_ATTN; m.index = cur(); m.cin1 = C; m.cout = C; m.res = res;
     const int T = res * res;
     m.tcattn = tcmode && (C % 128 == 0) && (T % 128 == 0) && (T <= 1024);
-    // fp16 operands: the logits/probabilities never leave the chip, so only the fused core is implemented
-    if (om == 2 && !tc_attn_supported(T, C, true)) m.tcattn = false;
+    // fp16 operands: the logits/probabilities never leave the chip, so only the fused core (T = 256) and the flash core
+    // (attn_flash.cu: T % 128 == 0 up to 4096, C = 128 / 256 / 512) are implemented
+    if (om == 2) m.tcattn = tc_attn_supported(T, C, true) || attn_flash_supported(T, C);
     // few tokens (T <= 64: the 4x4 block of CIFAR-10, the 8x8, 512-channel bottleneck of FFHQ-1024): one CTA per image
     // (attn_small_kernel); otherwise the block runs as separate contractions
     const bool small_ok = attn_small_supported(T, C);
@@ -914,8 +915,9 @@ struct Builder {
       });
       tfree(a);
       // Fused core (default): logits, softmax, P.V, NIN_3, residual, rescale and quad sums in one kernel; the
-      // [T,T] logits/probabilities and the attention output stay on chip; other token counts (tf32 mode) use separate launches.
-      if (om == 2 && !(tc && m.tc2 && tc_attn_supported(T, C, true))) {
+      // [T,T] logits/probabilities and the attention output stay on chip.  Other shapes: the flash core in fp16 operand mode
+      // (logits on chip, O through HBM into NIN_3), separate launches otherwise.
+      if (om == 2 && !(tc && m.tc2 && (tc_attn_supported(T, C, true) || attn_flash_supported(T, C)))) {
         set_error("ncsnpp: fp16 operand mode needs the fused attention core (T=%d C=%d)", T, C); rc = 2; return Tensor();
       }
       if (tc && m.tc2 && tc_attn_supported(T, C, om == 2) && !tan && !split) {
@@ -935,42 +937,54 @@ struct Builder {
         ffree(qk, qkb); ffree(vT, vtb);
         return out;
       }
-      float* S = falloc2(BT * T, &sb, &dS);
-      // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax (split TF32: q | k split once for both operands)
-      Pair qkp;
-      if (tc && split) qkp = split_pair(qk, (long long)B * T * 2 * C, "q|k");
-      const float* qkh = qkp.hi ? qkp.hi : qk;
-      gemm(tc, qkh, 2 * C, BT, T, qkh + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30,
-           qkp.lo, qkp.lo ? qkp.lo + C : nullptr);
-      release(qkp);
-      if (tan) {   // dS = dq k^T + q dk^T
-        long long tb; float* t1 = falloc(BT * T, &tb);
-        tangent([&] {
-          gemm(tc, dqk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, t1, T, nullptr, 1 << 30);
-          gemm(tc, qk, 2 * C, BT, T, dqk + C, 2 * C, BT, T, B, T, T, C, nullptr, t1, T, 1.f, 0, dS, T, nullptr, 1 << 30);
-        });
-        ffree(t1, tb);
+      if (om == 2) {   // flash core: logits, online softmax and P.V on chip; O (fp16) feeds NIN_3 below
+        O = falloc(BT * C, &ob);
+        if (!dry) {
+          AttnFlashPlan pl;
+          if (int r = attn_flash_plan(qk, vT, bqkv + 2 * C, O, B, T, C, &pl)) { rc = r; return Tensor(); }
+          name("attention flash T=%d C=%d (QK^T, online softmax, PV) [fused f16]", T, C);
+          next_bytes = (double)B * T * C * 2.0 * 4;   // q, k, v^T in, O out
+          op(1, [=](cudaStream_t st) { return attn_flash_launch(pl, st); }, 0, 4.0 * B * (double)T * T * C);
+        }
+        ffree(qk, qkb); ffree(vT, vtb);
+      } else {
+        float* S = falloc2(BT * T, &sb, &dS);
+        // logits[b][q][k] = q . k   (layerspp.py:82), scaled inside the softmax (split TF32: q | k split once for both operands)
+        Pair qkp;
+        if (tc && split) qkp = split_pair(qk, (long long)B * T * 2 * C, "q|k");
+        const float* qkh = qkp.hi ? qkp.hi : qk;
+        gemm(tc, qkh, 2 * C, BT, T, qkh + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, S, T, nullptr, 1 << 30,
+             qkp.lo, qkp.lo ? qkp.lo + C : nullptr);
+        release(qkp);
+        if (tan) {   // dS = dq k^T + q dk^T
+          long long tb; float* t1 = falloc(BT * T, &tb);
+          tangent([&] {
+            gemm(tc, dqk, 2 * C, BT, T, qk + C, 2 * C, BT, T, B, T, T, C, nullptr, nullptr, 0, 1.f, 0, t1, T, nullptr, 1 << 30);
+            gemm(tc, qk, 2 * C, BT, T, dqk + C, 2 * C, BT, T, B, T, T, C, nullptr, t1, T, 1.f, 0, dS, T, nullptr, 1 << 30);
+          });
+          ffree(t1, tb);
+        }
+        ffree(qk, qkb);
+        name("softmax T=%d", T);
+        const int prnd = tc ? om : 0;   // probabilities in the operand format of the P.V contraction (fp32 when split TF32)
+        op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, prnd, st); }, 4);
+        if (tan) {   // dP = P (sc dS - rowsum(P sc dS)), over dS
+          name("softmax_tangent T=%d", T);
+          tangent([&] { op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, prnd, st); }, 4); });
+        }
+        O = falloc2(BT * C, &ob, &dO);
+        // h[b][q][c] = sum_k P[q][k] v[k][c] + bv[c]   (layerspp.py:86)
+        gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? om : 0, O, C);
+        if (tan) {   // dO = dP v + P dv
+          long long tb; float* t2 = falloc(BT * C, &tb);
+          tangent([&] {
+            gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
+            gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? om : 0, dO, C);
+          });
+          ffree(t2, tb);
+        }
+        ffree(S, sb); ffree(vT, vtb);
       }
-      ffree(qk, qkb);
-      name("softmax T=%d", T);
-      const int prnd = tc ? om : 0;   // probabilities in the operand format of the P.V contraction (fp32 when split TF32)
-      op(1, [=](cudaStream_t st) { return launch_softmax_rows(S, S, (long long)Bc * T, T, sc, prnd, st); }, 4);
-      if (tan) {   // dP = P (sc dS - rowsum(P sc dS)), over dS
-        name("softmax_tangent T=%d", T);
-        tangent([&] { op(1, [=](cudaStream_t st) { return launch_softmax_tangent(S, dS, (long long)Bc * T, T, sc, prnd, st); }, 4); });
-      }
-      O = falloc2(BT * C, &ob, &dO);
-      // h[b][q][c] = sum_k P[q][k] v[k][c] + bv[c]   (layerspp.py:86)
-      gemm(tc, S, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, bqkv + 2 * C, nullptr, 0, 1.f, m.tc2 ? om : 0, O, C);
-      if (tan) {   // dO = dP v + P dv
-        long long tb; float* t2 = falloc(BT * C, &tb);
-        tangent([&] {
-          gemm(tc, dS, T, BT, T, vT, T, (long long)B * C, C, B, T, C, T, nullptr, nullptr, 0, 1.f, 0, t2, C);
-          gemm(tc, S, T, BT, T, dvT, T, (long long)B * C, C, B, T, C, T, nullptr, t2, C, 1.f, m.tc2 ? om : 0, dO, C);
-        });
-        ffree(t2, tb);
-      }
-      ffree(S, sb); ffree(vT, vtb);
     }
     Tensor out = talloc(C, x.H, x.W);
     Tensor Ot; Ot.p = O; Ot.C = C; Ot.H = x.H; Ot.W = x.W; Ot.d = dO;

@@ -159,6 +159,20 @@ int tc_attn_plan_create(const TcAttnDesc& d, TcAttnPlan** out);
 void tc_attn_plan_destroy(TcAttnPlan* p);
 int tc_attn_launch(const TcAttnPlan* p, cudaStream_t st);
 
+// ---- attn_flash.cu : flash-style fp16 attention core O = softmax(q k^T / sqrt(C)) v + b_v (online softmax, the logits
+// never leave the chip) for T % 128 == 0, 128 <= T <= 4096, C in {128, 256, 512}.  qk = [nimg*T][2C] (q | k), vT =
+// [nimg][C][T] (v^T without b_v), out = [nimg*T][C], all fp16; bv fp32.  The plan is a value (tensor maps + arguments).
+struct AttnFlashPlan {
+  CUtensorMap tmQ, tmK, tmV;
+  const float* bv;
+  void* out;
+  float logit_scale;        // C^-0.5 * log2(e)
+  int nimg, T, C;
+};
+bool attn_flash_supported(int T, int C);
+int attn_flash_plan(const void* qk, const void* vT, const float* bv, void* out, int nimg, int T, int C, AttnFlashPlan* pl);
+int attn_flash_launch(const AttnFlashPlan& p, cudaStream_t st);
+
 // ---- pc_update.cu -----------------------------------------------------------
 struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` elements
   unsigned long long seed;
