@@ -19,13 +19,13 @@
 //                produce_halo, three W-shifted copies of the tile with its halo per channel chunk;
 //   warps 1..3   idle (their registers go to the MMA warpgroups);
 //   warps 4..11  two MMA warpgroups, m64 x BN wgmma over 64 rows each: consume_ring or consume_halo per tile, then
-//                store_tile (NCHW head, frag_swap or frag_rows, compiled per residual x store format x stats).
+//                store_tile (NCHW head, or stage_epilogue - compiled per orientation x residual x store format x stats -
+//                through shared memory and TMA stores that drain during the next tile's mainloop).
 #include "tc_common.cuh"
 #include <cudaTypedefs.h>
 #include <array>
 #include <mutex>
 #include <cstring>
-#include <type_traits>
 
 namespace b200 {
 
@@ -35,14 +35,15 @@ namespace {
 // copies of the tile *with its one-row halo* (TMA box [chunk, W, rows + 2], origin w = -1 / 0 / +1, zero fill outside the
 // image); the operand of tap (dh, dw) is copy[dw] starting (dh + 1) * W pixels in - a multiple of 1024 bytes, so a plain
 // swizzled descriptor.  L2 -> shared-memory traffic per chunk: 3 x (rows + 2) / rows tiles instead of 9.
-constexpr int HALO_XS = 4;                  // halo copies in flight
+constexpr int HALO_XS = 3;                  // halo copies in flight (each feeds 3 K steps)
 constexpr int HALO_X_BYTES = 40 * 1024;     // swapped form: (8 + 2) rows x 32 pixels x 128 B
-constexpr int HALO_WS = 4;                  //   its weight-slice ring: 4 x 16 KB   (4 x 40 + 4 x 16 = 224 KB)
+constexpr int HALO_WS = 4;                  //   its weight-slice ring: 4 x 16 KB   (3 x 40 + 4 x 16 = 184 KB)
 
 struct TcParams {
   // [.][0] hi, [.][1] split-TF32 lo twin.  a: sources 0, 1 = the filter input, 2, 3 = the extra 1x1 K phase (fused skip
   // projection, weights w[1]); h: halo form, box [bke, W, tile rows + 2, 1].  Maps a plan lacks copy a[0] (w[1]: w[0]).
   CUtensorMap a[4][2], w[2][2], h[2][2];
+  CUtensorMap out_map, res_map;            // staged epilogue: [rows][N_total] output (store) and fp32 residual (load)
   int nphase;                              // 3: split TF32, every K step loads (A lo, W hi), (A hi, W lo), (A hi, W hi); else 1
   int halo;                               // 1: 3x3 taps read W-shifted halo copies of the tile (3 loads per channel chunk instead of 9)
   int halo_dh_bytes;                       // W * 128: bytes between the operand windows of consecutive filter rows inside a copy
@@ -69,6 +70,217 @@ __device__ __forceinline__ PhaseMaps phase_maps(const TcParams& p, const CUtenso
   return {&a[p.nphase == 3 && ph == 0], &w[ph == 1]};
 }
 
+
+// Staged epilogue.  Each MMA warpgroup owns two STG_BUF-byte shared-memory buffers and stores its 64 accumulator rows in
+// rounds: its warps write one round's values into a buffer, laid out as rows of the output, and one thread (the
+// warpgroup's leader) TMA-stores it while the warps fill the other buffer.  The last stores of a tile drain while the
+// next tile's mainloop runs.  A round is 32 output columns of the 64 rows (row-major tiles: one box of 64 pixels x 32
+// channels) or 32 pixels of the 64 output channels (swapped tiles: two boxes of 32 pixels x 32 channels).  Box rows hold
+// 32 elements: 128 B with the 128-byte swizzle for fp32 (output and residual), 64 B with the 64-byte swizzle for fp16
+// output, so the fragment writes do not bank-conflict.  The TMA store clips at the tensor map's bounds (the M tail, an
+// output pitch wider than N).  The residual of round r + 1 is TMA-loaded into the other buffer while round r is
+// computed (round 0 at tile start, before the mainloop), and each value's result overwrites its residual in place.
+// (Also prefetching a tile's later residual rounds into L2 at tile start measured slower on H100: 832 instead of 732 us
+// for `conv3x3 128->128 @32 +res` at batch 1024.)
+constexpr int STG_BUF = 8 * 1024;
+constexpr int STG_BYTES = 2 * 2 * STG_BUF;   // two warpgroups x two buffers
+
+// Read-only global load kept in program order with the epilogue's other asm (shared-memory accesses, barriers): the
+// compiler would otherwise hoist the bias / row-vector loads of later rounds and spill them next to the accumulator.
+__device__ __forceinline__ float2 ldg_f32x2_ordered(const float* a) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(a));
+  return v;
+}
+
+// byte offset of element (row r, column c) of a staged box with 32-element rows
+template <bool F16>
+__device__ __forceinline__ uint32_t stg_off(int r, int c) {
+  if (F16) return r * 64 + ((((c >> 3) ^ (r >> 1)) & 3) << 4) + (c & 7) * 2;
+  return r * 128 + ((((c >> 2) ^ r) & 7) << 4) + (c & 3) * 4;
+}
+
+// One warpgroup's output region in one tile, swapped (SWAP) or row-major: box k of round r starts at global
+// (column, row) (box_col(r, k), box_row(r)).
+template <bool SWAP>
+struct StageTile {
+  int col0, row0;
+  static constexpr int nbox() { return SWAP ? 2 : 1; }
+  __device__ __forceinline__ int box_col(int r, int k) const { return col0 + 32 * (SWAP ? k : r); }
+  __device__ __forceinline__ int box_row(int r) const { return row0 + (SWAP ? 32 * r : 0); }
+  static constexpr int box_bytes(int es) { return (SWAP ? 32 : 64) * 32 * es; }
+};
+
+template <int BN, bool SWAP>
+__device__ __forceinline__ StageTile<SWAP> stage_tile(const TcParams& p, int tile, int g) {
+  const int nt = tile % p.tiles_n, mg = tile / p.tiles_n;
+  if (SWAP) return {nt * 128 + 64 * g, mg * 256};
+  const int b = mg / p.tiles_m_per_batch, mt = mg % p.tiles_m_per_batch;
+  return {nt * BN, b * p.M_per_batch + mt * BM + 64 * g};
+}
+
+// Leader: the residual of round r into buffer `buf`, completing on `bar` (shared-window addresses).
+template <bool SWAP>
+__device__ __forceinline__ void load_residual(const TcParams& p, const StageTile<SWAP>& t, int r, uint32_t buf, uint32_t bar) {
+  mbar_expect_tx(bar, STG_BUF);
+  for (int k = 0; k < t.nbox(); ++k) tma_load_2d(&p.res_map, buf + k * t.box_bytes(4), bar, t.box_col(r, k), t.box_row(r));
+}
+
+// The epilogue of one warp's 16 accumulator rows, specialised by operand orientation (SWAP), residual add (RES), store
+// format (MODE: 0 fp32, 1 TF32-rounded fp32, 2 fp16) and GroupNorm quad sums of the stored values (STATS).  Each value is
+// (acc + (bias + rowvec) + residual) * scale, then rounded, as it always was; only where it is written changed.
+//   SWAP: rows = output channels c0 + 16wq .. of ONE image, columns = the tile's 256 pixels.  Lane l holds channels
+//         l/4 and l/4 + 8 of pixel pairs 8j + 2(l%4).
+//   else: rows = pixels / tokens, columns = output channels; lane l holds rows l/4 and l/4 + 8, column pairs 8j + 2(l%4).
+//         rows_valid: rows of the warp's 16 inside the matrix (GroupNorm sums only: the TMA store clips the rest).
+template <int BN, bool SWAP, bool RES, int MODE, bool STATS>
+__device__ __forceinline__ void stage_epilogue(const TcParams& p, const float (&d)[BN / 2], const StageTile<SWAP>& t, uint32_t stg,
+                                               uint32_t rbar, uint32_t& rpar, int rows_valid, int g, int wq, int lane,
+                                               bool leader) {
+  constexpr bool H = MODE == 2;
+  constexpr int ES = H ? 2 : 4;
+  constexpr int ROUNDS = SWAP ? 8 : BN / 32;
+  const Epilogue& e = p.epi;
+  const float scale = e.scale;
+  const int q = lane & 3;
+  // row-major: the warp's two rows in the box; swapped: its two channels in box wq / 2
+  const int ra = (SWAP ? 16 * (wq & 1) : 16 * wq) + (lane >> 2), rb = ra + 8;
+  const int kbox = SWAP ? wq >> 1 : 0;
+  const bool va = ra - 16 * wq < rows_valid, vb = rb - 16 * wq < rows_valid;
+  int img;
+  float adda = 0.f, addb = 0.f;
+  const float* rv = nullptr;
+  if (SWAP) {
+    img = t.row0 / e.rows_per_img;     // rows_per_img % 256 == 0: one image per tile
+    const int ca = t.col0 + 32 * kbox + ra, cb = ca + 8;
+    adda = (e.bias ? __ldg(e.bias + ca) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + ca) : 0.f);
+    addb = (e.bias ? __ldg(e.bias + cb) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + cb) : 0.f);
+  } else {
+    img = rows_valid > 0 ? (t.row0 + 16 * wq) / e.rows_per_img : 0;   // the 16 rows of a warp belong to one image
+    rv = e.rowvec ? e.rowvec + (long long)img * e.rowvec_ld : nullptr;
+  }
+  // Offsets of the thread's values in a box, output and fp32 residual layouts.  The swizzle repeats every 8 rows and
+  // only permutes 16-byte chunks within a row, so
+  //   swapped:   the four values of pixel rows 2q + {0, 1}; column group jj is 8jj rows further on;
+  //   row-major: rows ra and rb at column 2q; column group jj (8 columns = 2 fp32 / 1 fp16 chunks further) flips
+  //              chunk-index bits, i.e. XORs the offset with jj << 5 (fp32) or jj << 4 (fp16).
+  uint32_t ooff[SWAP ? 4 : 2], roff[SWAP ? 4 : 2];
+#pragma unroll
+  for (int i = 0; i < (SWAP ? 4 : 2); ++i) {
+    const int row = SWAP ? 2 * q + (i & 1) : (i ? rb : ra), col = SWAP ? (i < 2 ? ra : rb) : 2 * q;
+    ooff[i] = stg_off<H>(row, col);
+    roff[i] = stg_off<false>(row, col);
+  }
+  // writes the four values of fragment column group jj of the round: fp32, or fp16 pairs h01 = (v0, v1), h23 = (v2, v3)
+  // (cvt.rn.f16x2 rounds each half as cvt.rn.f16 does)
+  auto put = [&](uint32_t obox, int jj, const float* v, uint32_t h01, uint32_t h23) {
+    if (SWAP) {
+      if (H) {
+        st_shared_u16(obox + ooff[0] + jj * 8 * 64, (uint16_t)h01); st_shared_u16(obox + ooff[1] + jj * 8 * 64, (uint16_t)(h01 >> 16));
+        st_shared_u16(obox + ooff[2] + jj * 8 * 64, (uint16_t)h23); st_shared_u16(obox + ooff[3] + jj * 8 * 64, (uint16_t)(h23 >> 16));
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) st_shared_f32(obox + ooff[i] + jj * 8 * 128, v[i]);
+      }
+    } else if (H) {
+      st_shared_u32(obox + (ooff[0] ^ (jj << 4)), h01);
+      st_shared_u32(obox + (ooff[1] ^ (jj << 4)), h23);
+    } else {
+      st_shared_f32x2(obox + (ooff[0] ^ (jj << 5)), v[0], v[1]);
+      st_shared_f32x2(obox + (ooff[1] ^ (jj << 5)), v[2], v[3]);
+    }
+  };
+  float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
+#pragma unroll
+  for (int r = 0; r < ROUNDS; ++r) {
+    const int b = r & 1;
+    const uint32_t buf = stg + b * STG_BUF;
+    if (leader) {
+      bulk_wait_read<0>();   // the store of round r - 1 has read the other buffer
+      if (RES && r + 1 < ROUNDS) load_residual(p, t, r + 1, stg + (b ^ 1) * STG_BUF, rbar + 8 * (b ^ 1));
+    }
+    if (RES) { mbar_wait(rbar + 8 * b, (rpar >> b) & 1); rpar ^= 1u << b; }
+    const uint32_t rbox = buf + kbox * t.box_bytes(4);
+    const uint32_t obox = buf + kbox * t.box_bytes(ES);
+    // fp16 values overlay the round's fp32 residual: they are held, packed, until every thread has read its own
+    uint32_t hp[RES && H ? 8 : 1];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      const int j = 4 * r + jj;
+      float v[4];
+      if (SWAP) {
+        // pixel rows 8jj + 2q + {0, 1} of the box: the swizzle repeats every 8 rows, so 8jj rows past the jj = 0 offsets
+        v[0] = d[4 * j] + adda; v[1] = d[4 * j + 1] + adda; v[2] = d[4 * j + 2] + addb; v[3] = d[4 * j + 3] + addb;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          if (RES) v[i] += ld_shared_f32(rbox + roff[i] + jj * 1024);
+          v[i] *= scale;
+          if (MODE == 1) v[i] = round_tf32(v[i]);
+        }
+        if (STATS) {
+          sa += v[0] + v[1]; qa = fmaf(v[0], v[0], fmaf(v[1], v[1], qa));
+          sb += v[2] + v[3]; qb = fmaf(v[2], v[2], fmaf(v[3], v[3], qb));
+        }
+      } else {
+        const int col = t.col0 + 8 * j + 2 * q;
+        float2 ad = make_float2(0.f, 0.f);
+        if (e.bias) ad = ldg_f32x2_ordered(e.bias + col);
+        if (rv) { const float2 u = ldg_f32x2_ordered(rv + col); ad.x += u.x; ad.y += u.y; }
+        v[0] = d[4 * j] + ad.x; v[1] = d[4 * j + 1] + ad.y; v[2] = d[4 * j + 2] + ad.x; v[3] = d[4 * j + 3] + ad.y;
+        if (RES) {
+          const float2 ua = ld_shared_f32x2(rbox + (roff[0] ^ (jj << 5)));
+          const float2 ub = ld_shared_f32x2(rbox + (roff[1] ^ (jj << 5)));
+          v[0] += ua.x; v[1] += ua.y; v[2] += ub.x; v[3] += ub.y;
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          v[i] *= scale;
+          if (MODE == 1) v[i] = round_tf32(v[i]);
+        }
+        if (STATS) {
+          float s = (va ? v[0] + v[1] : 0.f) + (vb ? v[2] + v[3] : 0.f);
+          float qq = (va ? fmaf(v[0], v[0], v[1] * v[1]) : 0.f) + (vb ? fmaf(v[2], v[2], v[3] * v[3]) : 0.f);
+#pragma unroll
+          for (int m = 4; m <= 16; m <<= 1) { s += __shfl_xor_sync(0xffffffffu, s, m); qq += __shfl_xor_sync(0xffffffffu, qq, m); }
+          s += __shfl_xor_sync(0xffffffffu, s, 1); qq += __shfl_xor_sync(0xffffffffu, qq, 1);
+          if ((lane & ~2) == 0 && rows_valid > 0) {   // lanes 0 and 2: the two column quads of this 8-column group
+            double* qd = p.qstats + ((long long)img * (p.N_total >> 2) + (col >> 2)) * 2;
+            atomicAdd(qd, (double)s); atomicAdd(qd + 1, (double)qq);
+          }
+        }
+      }
+      const uint32_t h01 = H ? pack_half2(v[0], v[1]) : 0u, h23 = H ? pack_half2(v[2], v[3]) : 0u;
+      if constexpr (RES && H) { hp[2 * jj] = h01; hp[2 * jj + 1] = h23; }
+      else put(obox, jj, v, h01, h23);
+    }
+    if constexpr (RES && H) {
+      wg_barrier(g);
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) put(obox, jj, nullptr, hp[2 * jj], hp[2 * jj + 1]);
+    }
+    fence_async_smem();   // generic-proxy writes -> the TMA store's reads
+    wg_barrier(g);
+    if (leader) {
+      for (int k = 0; k < t.nbox(); ++k) tma_store_2d(&p.out_map, buf + k * t.box_bytes(ES), t.box_col(r, k), t.box_row(r));
+      bulk_commit();
+    }
+  }
+  if (SWAP && STATS) {
+#pragma unroll
+    for (int m = 1; m <= 8; m <<= 1) {   // pixel lanes (1, 2), then the four channels of a quad (4, 8)
+      sa += __shfl_xor_sync(0xffffffffu, sa, m); qa += __shfl_xor_sync(0xffffffffu, qa, m);
+      sb += __shfl_xor_sync(0xffffffffu, sb, m); qb += __shfl_xor_sync(0xffffffffu, qb, m);
+    }
+    if ((lane & 15) == 0) {
+      const int ca = t.col0 + 32 * kbox + ra, cb = ca + 8;
+      double* qd = p.qstats + ((long long)img * (p.N_total >> 2) + (ca >> 2)) * 2;
+      atomicAdd(qd, (double)sa); atomicAdd(qd + 1, (double)qa);
+      qd = p.qstats + ((long long)img * (p.N_total >> 2) + (cb >> 2)) * 2;
+      atomicAdd(qd, (double)sb); atomicAdd(qd + 1, (double)qb);
+    }
+  }
+}
+
 template <int BN>
 struct SmemLayout {
   static constexpr int STAGES = BN == 256 ? 4 : 6;
@@ -76,76 +288,17 @@ struct SmemLayout {
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int HALO_BYTES = HALO_XS * HALO_X_BYTES + HALO_WS * A_STAGE_BYTES;   // the swapped halo form's two rings
-  static constexpr int BAR_OFFSET = BN == 256 && HALO_BYTES > RING_BYTES ? HALO_BYTES : RING_BYTES;
+  static constexpr int STG_OFFSET = BN == 256 && HALO_BYTES > RING_BYTES ? HALO_BYTES : RING_BYTES;   // epilogue staging
+  static constexpr int BAR_OFFSET = STG_OFFSET + STG_BYTES;
+  // barrier arrays (byte offsets from the aligned base): ring full / empty, halo weight-slice full / empty, residual loads
+  static constexpr int FULL_BAR = BAR_OFFSET, EMPTY_BAR = FULL_BAR + 8 * STAGES, WFULL_BAR = EMPTY_BAR + 8 * STAGES;
+  static constexpr int WEMPTY_BAR = WFULL_BAR + 8 * HALO_WS, RES_BAR = WEMPTY_BAR + 8 * HALO_WS;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // barriers + slack for 1024-B alignment
   static_assert(TOTAL <= 232448, "exceeds the 227 KB shared-memory limit of sm_90");
   static_assert(BN != 256 || STAGES >= HALO_XS, "the halo copies use the first HALO_XS stage barriers");
+  static_assert(STG_OFFSET % 1024 == 0 && STG_BUF % 1024 == 0, "staged boxes need the 128-byte swizzle's 1024-B alignment");
+  static_assert(RES_BAR + 4 * 8 <= BAR_OFFSET + 256, "barriers overflow their 256 bytes");
 };
-
-// Epilogue of one warp's 16-channel x 256-pixel slice of a swapped tile (D^T = W X^T: rows = output channels, columns =
-// pixels of ONE image).  Lane l holds channels c0 + l/4 and c0 + l/4 + 8 of pixel pairs 8j + 2(l%4); eight lanes cover 32
-// contiguous bytes of a pixel's channel vector.
-template <bool RES, int MODE, bool STATS>
-__device__ __forceinline__ void frag_swap(const float (&d)[128], const Epilogue& e, double* qstats, int n_total,
-                                          int c0, long long pix0, int img, int lane) {
-  const int ca = c0 + (lane >> 2), cb = ca + 8;
-  const float adda = (e.bias ? __ldg(e.bias + ca) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + ca) : 0.f);
-  const float addb = (e.bias ? __ldg(e.bias + cb) : 0.f) + (e.rowvec ? __ldg(e.rowvec + img * e.rowvec_ld + cb) : 0.f);
-  const float scale = e.scale;
-  float sa = 0.f, qa = 0.f, sb = 0.f, qb = 0.f;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const long long px = pix0 + 8 * j + 2 * (lane & 3);
-    float o[4] = {d[4 * j] + adda, d[4 * j + 1] + adda, d[4 * j + 2] + addb, d[4 * j + 3] + addb};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const long long pix = px + (i & 1);
-      const int ch = i < 2 ? ca : cb;
-      if (RES) o[i] += __ldg(e.residual + pix * e.ld_res + ch);
-      o[i] *= scale;
-      if (MODE == 1) o[i] = round_tf32(o[i]);
-      if (MODE == 2) {
-        uint16_t h;
-        asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(o[i]));
-        reinterpret_cast<uint16_t*>(e.out)[pix * e.ld_out + ch] = h;
-      } else e.out[pix * e.ld_out + ch] = o[i];
-    }
-    if (STATS) {
-      sa += o[0] + o[1]; qa = fmaf(o[0], o[0], fmaf(o[1], o[1], qa));
-      sb += o[2] + o[3]; qb = fmaf(o[2], o[2], fmaf(o[3], o[3], qb));
-    }
-  }
-  if (STATS) {
-#pragma unroll
-    for (int m = 1; m <= 8; m <<= 1) {   // pixel lanes (1, 2), then the four channels of a quad (4, 8)
-      sa += __shfl_xor_sync(0xffffffffu, sa, m); qa += __shfl_xor_sync(0xffffffffu, qa, m);
-      sb += __shfl_xor_sync(0xffffffffu, sb, m); qb += __shfl_xor_sync(0xffffffffu, qb, m);
-    }
-    if ((lane & 15) == 0) {
-      double* qd = qstats + ((long long)img * (n_total >> 2) + (ca >> 2)) * 2;
-      atomicAdd(qd, (double)sa); atomicAdd(qd + 1, (double)qa);
-      qd = qstats + ((long long)img * (n_total >> 2) + (cb >> 2)) * 2;
-      atomicAdd(qd, (double)sb); atomicAdd(qd + 1, (double)qb);
-    }
-  }
-}
-
-// Calls f(RES, MODE, STATS) with the launch's residual add, store format (Epilogue::round_tf32) and GroupNorm quad sums as
-// std::integral_constant arguments: each of the 12 combinations is its own compiled epilogue.
-template <class F>
-__device__ __forceinline__ void dispatch_epilogue(const Epilogue& e, const double* qstats, F&& f) {
-  auto with_stats = [&](auto res, auto mode) {
-    if (qstats) f(res, mode, std::true_type{});
-    else f(res, mode, std::false_type{});
-  };
-  auto with_mode = [&](auto res) {
-    if (e.round_tf32 == 0) with_stats(res, std::integral_constant<int, 0>{});
-    else if (e.round_tf32 == 1) with_stats(res, std::integral_constant<int, 1>{});
-    else with_stats(res, std::integral_constant<int, 2>{});
-  };
-  if (e.residual) with_mode(std::true_type{});
-  else with_mode(std::false_type{});
-}
 
 // Producer stages run on warp 0 as a whole; only the elected lane (`issue`) issues TMA instructions.
 // Nine-load form, swapped or row-major: per K step one ring slot with the W box and the A box(es) shifted by the tap.
@@ -284,48 +437,50 @@ __device__ __forceinline__ void produce_halo(const TcParams& p, uint8_t* smem, u
 // MMA stages: warpgroup g (0, 1) owns accumulator rows 64g .. 64g + 63 of every tile.  A K step is released to the
 // producer once the wgmma after it has been issued (wait_group 1), so the tensor core always has the next step queued
 // while the previous one's slot is handed back.
+// The MMA warps address shared memory through 32-bit shared-window addresses (sm: the aligned base, SmemLayout
+// offsets): generic pointers would hold two registers each next to the 128-register accumulator.
 // One tile from the nine-load ring.
 template <int BN, bool F16>
-__device__ __forceinline__ void consume_ring(const TcParams& p, uint8_t* smem, float (&acc)[BN / 2], uint64_t* full_bar,
-                                             uint64_t* empty_bar, int kiters, uint32_t& stage, uint32_t& phase, int g, int lane) {
+__device__ __forceinline__ void consume_ring(const TcParams& p, uint32_t sm, float (&acc)[BN / 2], int kiters, uint32_t& stage,
+                                             uint32_t& phase, int g, int lane) {
   using L = SmemLayout<BN>;
   int pend = -1;
   for (int it = 0; it < kiters; ++it) {
-    mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
+    mbar_wait(sm + L::FULL_BAR + 8 * stage, phase);
+    const uint32_t sa = sm + stage * L::STAGE_BYTES;
     wgmma_kstep<BN, F16>(acc, make_smem_desc(sa + g * (A_STAGE_BYTES / 2)), make_smem_desc(sa + A_STAGE_BYTES), it);
     wgmma_wait<1>();
-    if (lane == 0 && pend >= 0) mbar_arrive(&empty_bar[pend]);
+    if (lane == 0 && pend >= 0) mbar_arrive(sm + L::EMPTY_BAR + 8 * pend);
     pend = (int)stage;
     if (++stage == L::STAGES) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
-  if (lane == 0 && pend >= 0) mbar_arrive(&empty_bar[pend]);
+  if (lane == 0 && pend >= 0) mbar_arrive(sm + L::EMPTY_BAR + 8 * pend);
 }
 
 // One tile of the halo form: A = the 16 KB weight slice (128 output channels), B = 256 pixel rows of a halo copy starting
 // one filter row (W pixels) further in per dh; the slice's slot is released per tap, the copy's after its three taps.
 template <int BN, bool F16>
-__device__ __forceinline__ void consume_halo(const TcParams& p, uint8_t* smem, float (&acc)[BN / 2], uint64_t* full_bar,
-                                             uint64_t* empty_bar, uint64_t* wfull_bar, uint64_t* wempty_bar, uint32_t& stage,
+__device__ __forceinline__ void consume_halo(const TcParams& p, uint32_t sm, float (&acc)[BN / 2], uint32_t& stage,
                                              uint32_t& phase, uint32_t& ws, uint32_t& wphase, int g, int lane) {
-  const uint32_t wring = smem_u32(smem + HALO_XS * HALO_X_BYTES);
+  using L = SmemLayout<BN>;
+  const uint32_t wring = sm + HALO_XS * HALO_X_BYTES;
   int it = 0, pend_ws = -1, pend_x = -1;
   for (int src = 0; src < 4; ++src) {
     const int nch = p.kchunks[src];
     const int ncopies = (src < 2 ? 3 * nch : nch) * p.nphase, ntap = src < 2 ? 3 : 1;
     for (int c = 0; c < ncopies; ++c) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint32_t sx = smem_u32(smem + stage * HALO_X_BYTES);
+      mbar_wait(sm + L::FULL_BAR + 8 * stage, phase);
+      const uint32_t sx = sm + stage * HALO_X_BYTES;
       for (int dhi = 0; dhi < ntap; ++dhi, ++it) {
-        mbar_wait(&wfull_bar[ws], wphase);
+        mbar_wait(sm + L::WFULL_BAR + 8 * ws, wphase);
         const uint64_t adesc = make_smem_desc(wring + ws * A_STAGE_BYTES + g * (A_STAGE_BYTES / 2));
         const uint64_t bdesc = make_smem_desc(sx + (src < 2 ? dhi * p.halo_dh_bytes : 0));
         wgmma_kstep<BN, F16>(acc, adesc, bdesc, it);
         wgmma_wait<1>();
         if (lane == 0) {
-          if (pend_ws >= 0) mbar_arrive(&wempty_bar[pend_ws]);
-          if (pend_x >= 0) mbar_arrive(&empty_bar[pend_x]);
+          if (pend_ws >= 0) mbar_arrive(sm + L::WEMPTY_BAR + 8 * pend_ws);
+          if (pend_x >= 0) mbar_arrive(sm + L::EMPTY_BAR + 8 * pend_x);
         }
         pend_ws = (int)ws; pend_x = dhi == ntap - 1 ? (int)stage : -1;
         if (++ws == HALO_WS) { ws = 0; wphase ^= 1; }
@@ -335,68 +490,107 @@ __device__ __forceinline__ void consume_halo(const TcParams& p, uint8_t* smem, f
   }
   wgmma_wait<0>();
   if (lane == 0) {
-    if (pend_ws >= 0) mbar_arrive(&wempty_bar[pend_ws]);
-    if (pend_x >= 0) mbar_arrive(&empty_bar[pend_x]);
+    if (pend_ws >= 0) mbar_arrive(sm + L::WEMPTY_BAR + 8 * pend_ws);
+    if (pend_x >= 0) mbar_arrive(sm + L::EMPTY_BAR + 8 * pend_x);
   }
 }
 
-// Epilogue of one tile: this warp's 16 accumulator rows, starting at tile row rw.
+// Epilogue of one tile: warp wq of MMA warpgroup g stores its 16 accumulator rows (tile rows 64g + 16wq ..).
+// Network head (swapped operands, NCHW store):
 template <int BN>
-__device__ __forceinline__ void store_tile(const TcParams& p, const float (&acc)[BN / 2], int tile, int rw, int lane) {
+__device__ __forceinline__ void store_head(const TcParams& p, const float (&acc)[BN / 2], int tile, int g, int wq, int lane) {
   const Epilogue& e = p.epi;
-  if constexpr (BN == 256) {
-    if (p.swap) {
-      // swapped operands (128-channel layers, 1x1 convolutions, the head): rows = output channels, columns = 256 pixels
-      const int c0 = (int)(tile % p.tiles_n) * 128 + rw;
-      const int pix0 = (tile / p.tiles_n) * 256;
-      const int img = pix0 / e.rows_per_img;     // rows_per_img % 256 == 0: one image per tile
-      if (e.out_nchw) {
-        // Network head (ncsnpp.py:374-380): the 128-row weight tile is zero-padded above the n_valid image channels;
-        // (acc + bias) / sigma[img] is written as NCHW
-        const float dv = e.per_img_div ? __ldg(e.per_img_div + img * e.div_stride) : 1.f;
-        const int hw = e.rows_per_img, pix_in_img = (int)(pix0 - (long long)img * hw);
+  // ncsnpp.py:374-380: the 128-row weight tile is zero-padded above the n_valid image channels; (acc + bias) / sigma[img]
+  // is written as NCHW
+  const int c0 = (int)(tile % p.tiles_n) * 128 + g * 64 + wq * 16;
+  const int pix0 = (tile / p.tiles_n) * 256;
+  const int img = pix0 / e.rows_per_img;     // rows_per_img % 256 == 0: one image per tile
+  const float dv = e.per_img_div ? __ldg(e.per_img_div + img * e.div_stride) : 1.f;
+  const int hw = e.rows_per_img, pix_in_img = (int)(pix0 - (long long)img * hw);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int co = c0 + (lane >> 2) + 8 * h;
-          if (co < e.n_valid) {
-            const float add = e.bias ? __ldg(e.bias + co) : 0.f;
-            float* dst = e.out + ((long long)img * e.n_valid + co) * hw + pix_in_img + 2 * (lane & 3);
+  for (int h = 0; h < 2; ++h) {
+    const int co = c0 + (lane >> 2) + 8 * h;
+    if (co < e.n_valid) {
+      const float add = e.bias ? __ldg(e.bias + co) : 0.f;
+      float* dst = e.out + ((long long)img * e.n_valid + co) * hw + pix_in_img + 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              *reinterpret_cast<float2*>(dst + 8 * j) = make_float2((acc[4 * j + 2 * h] + add) / dv, (acc[4 * j + 2 * h + 1] + add) / dv);
-          }
-        }
-      } else {
-        dispatch_epilogue(e, p.qstats, [&](auto res, auto mode, auto stats) {
-          frag_swap<decltype(res)::value, decltype(mode)::value, decltype(stats)::value>(acc, e, p.qstats, p.N_total, c0, pix0, img, lane);
-        });
-      }
-      return;
+      for (int j = 0; j < 32; ++j)
+        *reinterpret_cast<float2*>(dst + 8 * j) = make_float2((acc[4 * j + 2 * h] + add) / dv, (acc[4 * j + 2 * h + 1] + add) / dv);
     }
   }
-  const int nt = (int)(tile % p.tiles_n);
-  const int mg = tile / p.tiles_n;
-  const int b = (int)(mg / p.tiles_m_per_batch);
-  const int mt = (int)(mg % p.tiles_m_per_batch);
-  const int row0 = mt * BM + rw;
-  const int rows_valid = min(16, max(0, p.M_per_batch - row0));
-  const long long gm = (long long)b * p.M_per_batch + row0;
-  dispatch_epilogue(e, p.qstats, [&](auto res, auto mode, auto stats) {
-    frag_rows<BN, decltype(res)::value, decltype(mode)::value, decltype(stats)::value>(acc, e, p.qstats, p.N_total, gm, rows_valid, nt * BN, lane);
+}
+
+// Every other tile: the staged epilogue.
+template <int BN, bool SWAP, bool RES, int MODE, bool STATS>
+__device__ __forceinline__ void store_tile(const TcParams& p, const float (&acc)[BN / 2], int tile, int g, int wq, int lane,
+                                           uint32_t stg, uint32_t rbar, uint32_t& rpar, bool leader) {
+  const StageTile<SWAP> t = stage_tile<BN, SWAP>(p, tile, g);
+  const int mt = (int)((tile / p.tiles_n) % p.tiles_m_per_batch);
+  const int rows_valid = min(16, max(0, p.M_per_batch - (mt * BM + g * 64 + wq * 16)));   // row-major tiles only
+  stage_epilogue<BN, SWAP, RES, MODE, STATS>(p, acc, t, stg, rbar, rpar, rows_valid, g, wq, lane, leader);
+}
+
+// The MMA warps' tile loop.  store(acc, tile, stg, rbar, rpar, leader) is one compiled epilogue variant, chosen once
+// per launch: each variant's loop gets its own register allocation next to the 128-register accumulator.
+template <int BN, bool F16, class Store>
+__device__ __forceinline__ void gemm_tc_consumer(const TcParams& p, uint32_t sm, int g, int wq, int lane, Store&& store) {
+  using L = SmemLayout<BN>;
+  const int kiters = ((p.kchunks[0] + p.kchunks[1]) * p.taps + p.kchunks[2] + p.kchunks[3]) * p.nphase;
+  // the leader (thread 0 of the warpgroup: wq == 0, lane 0) issues the epilogue's TMA and owns its bulk groups; read from
+  // threadIdx where it is used rather than held across the loop
+  auto leader = [] { return (threadIdx.x & 127) == 0; };
+  const uint32_t stg = sm + L::STG_OFFSET + g * 2 * STG_BUF;   // this warpgroup's staging buffers
+  const uint32_t rbar = sm + L::RES_BAR + g * 2 * 8;            // and their residual barriers
+  uint32_t stage = 0, phase = 0, ws = 0, wphase = 0, rpar = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    if (leader() && p.epi.residual) {   // round 0's residual into buffer 0 (stg, rbar: the warpgroup's buffers, barriers)
+      if (BN == 256 && p.swap) load_residual(p, stage_tile<BN, true>(p, tile, g), 0, stg, rbar);
+      else load_residual(p, stage_tile<BN, false>(p, tile, g), 0, stg, rbar);
+    }
+    float acc[BN / 2];
+    if (BN == 256 && p.halo) consume_halo<BN, F16>(p, sm, acc, stage, phase, ws, wphase, g, lane);
+    else consume_ring<BN, F16>(p, sm, acc, kiters, stage, phase, g, lane);
+    store(acc, tile, stg, rbar, rpar, leader());
+  }
+  if (leader()) bulk_wait<0>();   // every store has landed before the CTA exits (dependent launches run under PDL)
+}
+
+// The tile loop with one staged-epilogue variant.  (Functions and by-value captures throughout: a lambda object or a
+// captured reference that is not inlined away lives in local memory.)
+template <int BN, bool F16, bool SWAP, bool RES, int MODE, bool STATS>
+__device__ __forceinline__ void gemm_tc_staged(const TcParams& p, uint32_t sm, int g, int wq, int lane) {
+  gemm_tc_consumer<BN, F16>(p, sm, g, wq, lane, [&p, g, wq, lane](const float (&acc)[BN / 2], int tile, uint32_t stg,
+                                                                uint32_t rbar, uint32_t& rpar, bool leader) {
+    store_tile<BN, SWAP, RES, MODE, STATS>(p, acc, tile, g, wq, lane, stg, rbar, rpar, leader);
   });
 }
 
-template <int BN, bool F16>
-__device__ __forceinline__ void gemm_tc_consumer(const TcParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                                 uint64_t* wfull_bar, uint64_t* wempty_bar, int g, int wq, int lane) {
-  const int kiters = ((p.kchunks[0] + p.kchunks[1]) * p.taps + p.kchunks[2] + p.kchunks[3]) * p.nphase;
-  uint32_t stage = 0, phase = 0, ws = 0, wphase = 0;
-  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-    float acc[BN / 2];
-    if (BN == 256 && p.halo) consume_halo<BN, F16>(p, smem, acc, full_bar, empty_bar, wfull_bar, wempty_bar, stage, phase, ws, wphase, g, lane);
-    else consume_ring<BN, F16>(p, smem, acc, full_bar, empty_bar, kiters, stage, phase, g, lane);
-    store_tile<BN>(p, acc, tile, g * 64 + wq * 16, lane);
+// Staged-epilogue variant v = 6 RES + 2 MODE + STATS (residual add, store format Epilogue::round_tf32, GroupNorm quad
+// sums): each of the 12 is its own compiled tile loop.
+template <int BN, bool F16, bool SWAP, int V = 0>
+__device__ __forceinline__ void gemm_tc_select(const TcParams& p, uint32_t sm, int g, int wq, int lane, int v) {
+  if constexpr (V < 12) {
+    if (v == V) gemm_tc_staged<BN, F16, SWAP, (V >= 6), (V / 2) % 3, (V & 1) != 0>(p, sm, g, wq, lane);
+    else gemm_tc_select<BN, F16, SWAP, V + 1>(p, sm, g, wq, lane, v);
   }
+}
+
+// Selects the epilogue (head, or orientation x staged variant) and runs the tile loop.
+template <int BN, bool F16>
+__device__ __forceinline__ void gemm_tc_mma(const TcParams& p, uint32_t sm, int g, int wq, int lane) {
+  if constexpr (BN == 256) {
+    if (p.swap && p.epi.out_nchw) {
+      gemm_tc_consumer<BN, F16>(p, sm, g, wq, lane, [&p, g, wq, lane](const float (&acc)[BN / 2], int tile, uint32_t, uint32_t, uint32_t&, bool) {
+        store_head<BN>(p, acc, tile, g, wq, lane);
+      });
+      return;
+    }
+  }
+  const int v = (p.epi.residual ? 6 : 0) + 2 * p.epi.round_tf32 + (p.qstats ? 1 : 0);
+  if constexpr (BN == 256) {
+    if (p.swap) { gemm_tc_select<BN, F16, true>(p, sm, g, wq, lane, v); return; }
+  }
+  gemm_tc_select<BN, F16, false>(p, sm, g, wq, lane, v);
 }
 
 // ---------------------------------------------------------------------------
@@ -408,10 +602,11 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
   constexpr int STAGES = L::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* wfull_bar = empty_bar + STAGES;      // halo form: the weight-slice ring has its own barriers
-  uint64_t* wempty_bar = wfull_bar + HALO_WS;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::FULL_BAR);
+  uint64_t* empty_bar = reinterpret_cast<uint64_t*>(smem + L::EMPTY_BAR);
+  uint64_t* wfull_bar = reinterpret_cast<uint64_t*>(smem + L::WFULL_BAR);     // halo form: the weight-slice ring has its own barriers
+  uint64_t* wempty_bar = reinterpret_cast<uint64_t*>(smem + L::WEMPTY_BAR);
+  uint64_t* res_bar = reinterpret_cast<uint64_t*>(smem + L::RES_BAR);         // staged epilogue: residual loads, two per MMA warpgroup
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp index provably warp-uniform
 
@@ -419,6 +614,7 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
     // empty slots: one arrival per MMA warp (8)
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     for (int s = 0; s < HALO_WS; ++s) { mbar_init(&wfull_bar[s], 1); mbar_init(&wempty_bar[s], 8); }
+    for (int s = 0; s < 4; ++s) mbar_init(&res_bar[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -434,8 +630,8 @@ __global__ void __launch_bounds__(384, 1) gemm_tc_kernel(const __grid_constant__
   } else {
     regs_consumer();
     const int g = (warp >> 2) - 1, wq = warp & 3;   // MMA warpgroup and warp within it
-    if (p.f16) gemm_tc_consumer<BN, true>(p, smem, full_bar, empty_bar, wfull_bar, wempty_bar, g, wq, lane);
-    else gemm_tc_consumer<BN, false>(p, smem, full_bar, empty_bar, wfull_bar, wempty_bar, g, wq, lane);
+    if (p.f16) gemm_tc_mma<BN, true>(p, smem_u32(smem), g, wq, lane);
+    else gemm_tc_mma<BN, false>(p, smem_u32(smem), g, wq, lane);
   }
 }
 
@@ -458,14 +654,14 @@ PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
 }  // namespace
 
 int encode_map(CUtensorMap* tm, const float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-               const uint32_t* box, const uint32_t* elem_strides, bool f16) {
+               const uint32_t* box, const uint32_t* elem_strides, bool f16, CUtensorMapSwizzle swizzle) {
   auto fn = get_encode_fn();
   B200_REQUIRE(fn != nullptr, "gemm_tc: cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
   B200_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "gemm_tc: operand base %p not 16-byte aligned", (const void*)base);
   uint32_t estr[5] = {1, 1, 1, 1, 1};
   if (elem_strides) for (int i = 0; i < rank; ++i) estr[i] = elem_strides[i];
   CUresult r = fn(tm, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<float*>(base), dims,
-                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   B200_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled failed with CUresult %d "
                "(rank %d dims %llu,%llu,%llu,%llu box %u,%u,%u,%u)", (int)r, rank,
@@ -524,7 +720,11 @@ bool tc_gemm_supported(const TcGemmDesc& d, const char** why) {
   // a 32-row epilogue block spans two images only for 4x4 images (rows_per_img == 16)
   if ((d.qstats || d.epi.rowvec) && !(d.epi.rows_per_img % 32 == 0 || d.epi.rows_per_img == 16)) return fail("per-image epilogue terms need rows_per_img % 32 == 0 or == 16");
   if (d.epi.ld_out % 4 || (d.epi.residual && d.epi.ld_res % 4)) return fail("output pitch must be a multiple of 4 elements");
+  if (d.epi.round_tf32 < 0 || d.epi.round_tf32 > 2) return fail("store format must be 0 (fp32), 1 (TF32 grid) or 2 (fp16)");
   if (d.epi.round_tf32 == 2 && d.epi.ld_out % 8) return fail("fp16 output pitch must be a multiple of 8 elements");
+  // the epilogue's TMA store and residual load
+  if (!d.epi.out_nchw && (reinterpret_cast<uintptr_t>(d.epi.out) & 15)) return fail("output must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(d.epi.residual) & 15) return fail("residual must be 16-byte aligned");
   if (d.split && d.f16) return fail("split TF32 takes TF32 operands, not fp16");
   if (d.split && (!d.a1_lo || (d.a2 && !d.a2_lo) || (d.a3 && !d.a3_lo) || (d.a4 && !d.a4_lo) || !d.w_lo || (d.a3 && !d.w2_lo)))
     return fail("split TF32 needs the lo twin of every operand");
@@ -667,6 +867,21 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
     const uint64_t dims2[2] = {K3, (uint64_t)d.N_total};
     const uint64_t str2[1] = {K3 * es};
     if (int r = encode_pair(p.w[1], d.w2, d.w2_lo, 2, dims2, str2, wbox, nullptr)) return r;
+  }
+  // staged epilogue: the output and the residual as [rows][N_total] matrices of pitch ld_out / ld_res, in the epilogue's
+  // boxes (32 columns x 64 rows, or x 32 pixels in the swapped form); rows past M and columns past N are clipped
+  if (!d.epi.out_nchw) {
+    const uint64_t rows = d.conv ? (uint64_t)d.nimg * d.H * d.W : (uint64_t)d.nbatch * d.M_per_batch;
+    const uint64_t dims[2] = {(uint64_t)d.N_total, rows};
+    const uint32_t box[2] = {32, form.swap ? 32u : 64u};
+    const bool oh = d.epi.round_tf32 == 2;
+    const uint64_t ostr[1] = {(uint64_t)d.epi.ld_out * (oh ? 2 : 4)};
+    if (int r = encode_map(&p.out_map, d.epi.out, 2, dims, ostr, box, nullptr, oh, oh ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B))
+      return r;
+    if (d.epi.residual) {
+      const uint64_t rstr[1] = {(uint64_t)d.epi.ld_res * 4};
+      if (int r = encode_map(&p.res_map, d.epi.residual, 2, dims, rstr, box, nullptr, false)) return r;
+    }
   }
   // the maps the plan does not have (the kernel never reads them) copy a[0], or w[0]
   for (int s = 1; s < 4; ++s)

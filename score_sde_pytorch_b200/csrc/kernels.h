@@ -94,9 +94,11 @@ bool conv_lowc_supported(const SimtConv& p);
 int launch_conv_lowc(const SimtConv& p, cudaStream_t st);
 
 // ---- gemm_tc.cu : wgmma / TMA implicit GEMM (TF32 or fp16 operands) --------
-// TMA tensor map (SWIZZLE_128B, zero out-of-bounds fill) over fp32 or fp16 elements; also used by attn_tc.cu
+// TMA tensor map (SWIZZLE_128B unless told otherwise, zero out-of-bounds fill) over fp32 or fp16 elements; also used by
+// attn_tc.cu and attn_flash.cu
 int encode_map(CUtensorMap* tm, const float* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-               const uint32_t* box, const uint32_t* elem_strides = nullptr, bool f16 = false);
+               const uint32_t* box, const uint32_t* elem_strides = nullptr, bool f16 = false,
+               CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 int num_sms();   // of the current device
 struct TcGemmPlan;   // opaque, owns the encoded tensor maps
 struct TcGemmDesc {
