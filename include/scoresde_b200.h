@@ -82,6 +82,22 @@ B200_API int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int
                                      int batch, int h, int w, const float* w_packed, const float* bias,
                                      const float* w_skip, const float* bias_skip, int c_out, const float* residual,
                                      float scale, int round_tf32, float* out, void* stream);
+/* NCSNv2 building blocks on NHWC fp32 tensors (kernel tests; the engine's family 2 plans the same kernels).
+ * Dilated 3x3 'same' convolution (padding = dilation), out = conv + bias (+ residual), stored in mode round_out
+ * (0 fp32, 1 TF32 grid, 2 fp16 - tensor-core impls only); w_packed as b200_pack_conv_weight_f32 (ksize 3).
+ * impl 0 = CUDA cores (strict fp32), 1 = tensor cores on TF32-grid operands, 2 = tensor cores on fp16 operands. */
+B200_API int b200_conv_dilated_nhwc_f32(const float* x, int c, int batch, int h, int w, const float* w_packed, const float* bias,
+                                        int c_out, int dilation, const float* residual, int round_out, float* out, int impl,
+                                        void* stream);
+/* InstanceNorm2dPlus (models/normalization.py:157-183, eps 1e-5) of x [batch][hw][c], then ELU when act, stored in mode
+ * round_out; stats_ws holds batch * c * 66 doubles (the [batch][c][2] sums and up to 32 pixel slices of partial sums). */
+B200_API int b200_instnorm_plus_nhwc_f32(const float* x, int batch, int hw, int c, const float* alpha, const float* gamma,
+                                         const float* beta, int act, int round_out, float* y, double* stats_ws, void* stream);
+/* nn.MaxPool2d(5, stride 1, padding 2) of x [batch][h][w][c] into y (mode round_out); with add: sum = x + add */
+B200_API int b200_maxpool5_nhwc_f32(const float* x, int batch, int h, int w, int c, int round_out, float* y, const float* add,
+                                    float* sum, void* stream);
+/* acc [batch][h][w][c] += F.interpolate(lo [batch][hl][wl][c], (h, w), mode='bilinear', align_corners=True) */
+B200_API int b200_bilinear_add_nhwc_f32(const float* lo, int batch, int hl, int wl, int c, float* acc, int h, int w, void* stream);
 B200_API int b200_pack_conv_weight_f32(const float* w_oihw, float* w_packed, int c_out, int c_in, int ksize,
                                        int round_tf32, void* stream);
 /* Fused attention core of AttnBlockpp (layerspp.py:82-91) for T=256 tokens x C=256 channels per image, or T=256 x
@@ -162,7 +178,14 @@ typedef struct {
                                  * attn_resolutions, centered and the execution fields (precision, keep_activations, lanes,
                                  * cuda_core_head, pdl, no_halo, tangent); it requires
                                  * conditional = 1 and scale_by_sigma = 0, and ignores skip_rescale, progressive_input, progressive,
-                                 * fir_taps / fir_kernel, naive_resample and embedding_type. */
+                                 * fir_taps / fir_kernel, naive_resample and embedding_type.
+                                 * 2 = NCSNv2 (models/ncsnv2.py: NCSNv2 'ncsnv2_64' with num_levels = 4, NCSNv2_128 with
+                                 * num_levels = 5): ResidualBlocks with InstanceNorm2dPlus + ELU, dilated 3x3 convolutions and
+                                 * ConvMeanPool, RefineBlocks (RCU, MSF with bilinear sums, CRP with 5x5 max pooling), output
+                                 * divided by the per-image label, which the caller sets to sigmas[y].  Family 2 reads image_size,
+                                 * num_channels, nf, num_levels, centered and the execution fields; it ignores the rest, refuses
+                                 * tangent = 1 and precision = 3, and records module taps as 0 = begin_conv, then every
+                                 * ResidualBlock, then every RefineBlock in forward order. */
   int tangent;                  /* 0 (default): the forward alone.  1: the plan also carries the forward-mode tangent pass of
                                  * b200_ncsnpp_jvp: after each op its tangent op (the same contraction on the tangent buffers
                                  * without bias and time-embedding row, or a GroupNorm(+SiLU) / softmax tangent kernel).  Taken

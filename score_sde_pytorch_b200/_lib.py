@@ -64,6 +64,12 @@ SIGNATURES = {
   'b200_attention_core_f32': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int, c_int, c_int, c_float, c_int, c_void_p]),
   'b200_attention_flash_f16': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+  'b200_conv_dilated_nhwc_f32': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                         c_int, c_void_p, c_int, c_void_p]),
+  'b200_instnorm_plus_nhwc_f32': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                          c_void_p, c_void_p]),
+  'b200_maxpool5_nhwc_f32': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+  'b200_bilinear_add_nhwc_f32': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
   'b200_pack_conv_weight_f32': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
   'b200_gemm_nt_f32': (c_int, [c_void_p, c_ll, c_int, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_int, c_void_p, c_ll, c_int, c_void_p]),

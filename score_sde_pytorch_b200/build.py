@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libscoresde_b200.so')
 STAMP = os.path.join(HERE, '.libscoresde_b200.stamp')
-SOURCES = ['api.cu', 'elementwise.cu', 'conv_simt.cu', 'conv_lowc.cu', 'gemm_tc.cu', 'attn_tc.cu', 'attn_flash.cu', 'pc_update.cu', 'engine.cu', 'ode.cu', 'losses.cu', 'tangent.cu']
+SOURCES = ['api.cu', 'elementwise.cu', 'conv_simt.cu', 'conv_lowc.cu', 'gemm_tc.cu', 'attn_tc.cu', 'attn_flash.cu', 'pc_update.cu', 'engine.cu', 'ode.cu', 'losses.cu', 'tangent.cu', 'ncsnv2.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC,-fvisibility=hidden', '--expt-relaxed-constexpr']
 

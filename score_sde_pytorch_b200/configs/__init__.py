@@ -278,3 +278,71 @@ def subvp_celebahq_256_ddpmpp_continuous():
   c.model.num_res_blocks = 2
   c.model.attn_resolutions = (16,)
   return c
+
+
+def ve_cifar10_ncsnv2():
+  """``configs/ve/ncsnv2/cifar10.py`` — NCSNv2 (``model.name = 'ncsnv2_64'``): InstanceNorm++, ELU, nf=128, 232 noise
+  levels, discrete time (``continuous=False``) with annealed Langevin dynamics (predictor ``none``, corrector ``ald``,
+  5 steps per level, snr 0.176).  ``data.channels`` mirrors ``data.num_channels``: the reference's NCSNv2 constructor
+  reads that name (models/ncsnv2.py:55)."""
+  c = cifar10_defaults()
+  c.training.sde = 'vesde'
+  c.training.continuous = False
+  c.sampling.method = 'pc'
+  c.sampling.predictor = 'none'
+  c.sampling.corrector = 'ald'
+  c.sampling.n_steps_each = 5
+  c.sampling.snr = 0.176
+  c.data.channels = c.data.num_channels
+  m = c.model
+  m.name = 'ncsnv2_64'
+  m.scale_by_sigma = True
+  m.num_scales = 232
+  m.ema_rate = 0.999
+  m.normalization = 'InstanceNorm++'
+  m.nonlinearity = 'elu'
+  m.nf = 128
+  m.interpolation = 'bilinear'
+  c.optim = ConfigDict(weight_decay=0, optimizer='Adam', lr=1e-4, beta1=0.9, amsgrad=False, eps=1e-8, warmup=0, grad_clip=-1.)
+  return c
+
+
+def ve_celeba_ncsnv2():
+  """``configs/ve/ncsnv2/celeba.py`` over ``configs/default_celeba_configs.py``: the same network at 64x64, sigma_max 90,
+  500 noise levels, snr 0.128."""
+  c = ve_cifar10_ncsnv2()
+  c.data.dataset = 'CELEBA'
+  c.data.image_size = 64
+  c.model.sigma_max = 90.
+  c.model.num_scales = 500
+  c.sampling.snr = 0.128
+  return c
+
+
+def ve_bedroom_ncsnv2():
+  """``configs/ve/ncsnv2/bedroom.py`` over ``configs/default_lsun_configs.py``: NCSNv2_128 (``model.name = 'ncsnv2_128'``)
+  at 128x128, sigma_max 190, 1086 noise levels, 3 Langevin steps per level, snr 0.095, EMA 0.9999."""
+  c = ve_cifar10_ncsnv2()
+  c.data.dataset = 'LSUN'
+  c.data.category = 'bedroom'
+  c.data.image_size = 128
+  c.training.batch_size = 128
+  c.eval.batch_size = 512
+  c.sampling.n_steps_each = 3
+  c.sampling.snr = 0.095
+  m = c.model
+  m.name = 'ncsnv2_128'
+  m.sigma_max = 190
+  m.sigma_min = 0.01
+  m.num_scales = 1086
+  m.ema_rate = 0.9999
+  return c
+
+
+def tiny_ncsnv2(nf=32, image_size=16, num_scales=20):
+  """A small NCSNv2 (``ncsnv2_64`` walk; test fixture sized, not a reference config)."""
+  c = ve_cifar10_ncsnv2()
+  c.model.nf = nf
+  c.model.num_scales = num_scales
+  c.data.image_size = image_size
+  return c

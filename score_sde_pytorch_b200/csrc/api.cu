@@ -123,6 +123,47 @@ int b200_conv_nhwc_f32(const float* x1, int c1, const float* x2, int c2, int bat
   return launch_conv_simt(s, st);
 }
 
+int b200_conv_dilated_nhwc_f32(const float* x, int c, int batch, int h, int w, const float* w_packed, const float* bias,
+                               int c_out, int dilation, const float* residual, int round_out, float* out, int impl,
+                               void* stream) {
+  B200_REQUIRE(x && w_packed && out && dilation >= 1, "conv_dilated_nhwc: bad argument");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Epilogue ep; memset(&ep, 0, sizeof(ep));
+  ep.bias = bias; ep.residual = residual; ep.ld_res = c_out; ep.scale = 1.f; ep.round_tf32 = round_out;
+  ep.rows_per_img = h * w; ep.out = out; ep.ld_out = c_out;
+  if (impl == 1 || impl == 2) {
+    TcGemmDesc d; memset(&d, 0, sizeof(d));
+    d.f16 = impl == 2; d.a1 = x; d.C1 = c; d.conv = 1; d.H = h; d.W = w; d.nimg = batch; d.taps = 9; d.dilation = dilation;
+    d.w = w_packed; d.N_total = c_out; d.K_total = c; d.w_rows = 9LL * c_out; d.nbatch = 1; d.epi = ep;
+    TcGemmPlan* pl = nullptr;
+    if (int r = tc_gemm_plan_create(d, &pl)) return r;
+    const int r = tc_gemm_launch(pl, st);
+    tc_gemm_plan_destroy(pl);
+    return r;
+  }
+  B200_REQUIRE(impl == 0, "conv_dilated_nhwc: impl %d unknown", impl);
+  SimtConv s; memset(&s, 0, sizeof(s));
+  s.x1 = x; s.C1 = c; s.in_scale = 1.f; s.H = h; s.W = w; s.R = s.S = 3; s.stride = 1; s.pad = dilation; s.dilation = dilation;
+  s.OH = h; s.OW = w; s.nbatch = batch; s.a_batched = 1; s.w = w_packed; s.N = c_out; s.epi = ep;
+  return launch_conv_simt(s, st);
+}
+
+int b200_instnorm_plus_nhwc_f32(const float* x, int batch, int hw, int c, const float* alpha, const float* gamma,
+                                const float* beta, int act, int round_out, float* y, double* stats_ws, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (int r = launch_in_stats(x, batch, hw, c, stats_ws, st)) return r;
+  return launch_in_apply(x, stats_ws, alpha, gamma, beta, batch, hw, c, 1e-5f, act, round_out, y, st);
+}
+
+int b200_maxpool5_nhwc_f32(const float* x, int batch, int h, int w, int c, int round_out, float* y, const float* add, float* sum,
+                           void* stream) {
+  return launch_maxpool5(x, batch, h, w, c, round_out, y, add, sum, static_cast<cudaStream_t>(stream));
+}
+
+int b200_bilinear_add_nhwc_f32(const float* lo, int batch, int hl, int wl, int c, float* acc, int h, int w, void* stream) {
+  return launch_bilinear_add(lo, batch, hl, wl, c, acc, h, w, static_cast<cudaStream_t>(stream));
+}
+
 int b200_conv_skip_nhwc_f32(const float* x, int c, const float* s1, int cs1, const float* s2, int cs2, int batch, int h,
                             int w, const float* w_packed, const float* bias, const float* w_skip,
                             const float* bias_skip, int c_out, const float* residual, float scale, int round_tf32,

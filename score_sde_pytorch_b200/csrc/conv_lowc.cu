@@ -306,7 +306,7 @@ bool aligned(const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q
 bool conv_lowc_supported(const SimtConv& p) {
   const bool geom = (p.R == 3 && p.S == 3 && p.pad == 1) || (p.R == 1 && p.S == 1 && p.pad == 0);
   const long long ld1 = p.ld1 ? p.ld1 : p.C1, ld2 = p.ld2 ? p.ld2 : p.C2, wld = p.w_ld ? p.w_ld : p.C1 + p.C2;
-  return geom && p.stride == 1 && !p.in_nchw && p.in_scale == 1.f && p.in_shift == 0.f && p.OH == p.H && p.OW == p.W &&
+  return geom && p.stride == 1 && p.dilation <= 1 && !p.in_nchw && p.in_scale == 1.f && p.in_shift == 0.f && p.OH == p.H && p.OW == p.W &&
          p.H % LC_TH == 0 && p.W % LC_TW == 0 && p.C1 > 0 && p.C1 % LC_KC == 0 && p.C2 >= 0 && p.C2 % LC_KC == 0 &&
          (p.N == 16 || p.N == 32 || p.N == 64) && p.a_batched && p.w_batch_stride == 0 && ld1 % 4 == 0 && ld2 % 4 == 0 &&
          wld % 4 == 0 && !p.epi.out_nchw && !p.epi.per_img_div && (p.epi.round_tf32 == 0 || p.epi.round_tf32 == 1) &&

@@ -35,6 +35,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtConv p) {
   const long long ld1 = p.ld1 ? p.ld1 : p.C1, ld2 = p.ld2 ? p.ld2 : p.C2, wld = p.w_ld ? p.w_ld : Cin;
   const bool vecA = !p.in_nchw && (p.C1 % 4 == 0) && (p.C2 % 4 == 0) && (ld1 % 4 == 0) && (ld2 % 4 == 0);
   const bool vecB = (Cin % 4 == 0) && (wld % 4 == 0);
+  const int dil = p.dilation > 1 ? p.dilation : 1;   // filter tap spacing (the NCSNv2 dilated blocks)
 
   for (long long tile = blockIdx.x; tile < tiles_total; tile += gridDim.x) {
     const int nt = (int)(tile % tiles_n);
@@ -70,7 +71,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtConv p) {
         if (oy >= 0 && kk < K) {
           if (vecA) {
             const int tap = kk / Cin, c = kk % Cin;
-            const int iy = oy * p.stride + tap / p.S - p.pad, ix = s_ox[i] * p.stride + tap % p.S - p.pad;
+            const int iy = oy * p.stride + (tap / p.S) * dil - p.pad, ix = s_ox[i] * p.stride + (tap % p.S) * dil - p.pad;
             if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
               const long long pix = (long long)iy * p.W + ix;
               const float4 q = (c < p.C1) ? __ldg(reinterpret_cast<const float4*>(a1 + pix * ld1 + c))
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const SimtConv p) {
               const int k = kk + j;
               if (k >= K) break;
               const int tap = k / Cin, c = k % Cin;
-              const int iy = oy * p.stride + tap / p.S - p.pad, ix = s_ox[i] * p.stride + tap % p.S - p.pad;
+              const int iy = oy * p.stride + (tap / p.S) * dil - p.pad, ix = s_ox[i] * p.stride + (tap % p.S) * dil - p.pad;
               if (iy >= 0 && iy < p.H && ix >= 0 && ix < p.W) {
                 float t;
                 if (p.in_nchw) t = __ldg(a1 + ((long long)c * p.H + iy) * p.W + ix);   // same per-image offset

@@ -17,7 +17,9 @@ using namespace b200;
 namespace {
 
 // M_DOWN / M_UP: the DDPM family's Downsample / Upsample with_conv (layers.py:584-616)
-enum ModKind { M_FOURIER, M_LINEAR, M_CONV_IN, M_RESBLOCK, M_ATTN, M_PYR_DOWN, M_GN_OUT, M_CONV_OUT, M_COMBINE, M_DOWN, M_UP };
+// M_NRES / M_NREF / M_NHEAD: the NCSNv2 family's ResidualBlock, RefineBlock and output head (models/ncsnv2.py, layers.py)
+enum ModKind { M_FOURIER, M_LINEAR, M_CONV_IN, M_RESBLOCK, M_ATTN, M_PYR_DOWN, M_GN_OUT, M_CONV_OUT, M_COMBINE, M_DOWN, M_UP,
+               M_NRES, M_NREF, M_NHEAD };
 enum PackKind { PK_COPY = 0, PK_CONV = 1, PK_NIN = 2, PK_CONV_FLAT32 = 3, PK_CONV_PAD128 = 4 };
 
 struct Param {
@@ -37,6 +39,14 @@ struct Mod {
   int gn0w = -1, gn0b = -1, c0w = -1, c0b = -1, dw = -1, db = -1, gn1w = -1, gn1b = -1, c1w = -1, c1b = -1, c2w = -1, c2b = -1;
   int nw[4] = {-1, -1, -1, -1}, nb[4] = {-1, -1, -1, -1};
   int w = -1, b = -1;
+  // NCSNv2 (family 2).  M_NRES: dilation, InstanceNorm2dPlus parameters in[k] = {alpha, gamma, beta} of normalize1 (k = 0)
+  // and normalize2 (k = 1), conv1 (c0w, c0b), conv2 (c1w, c1b), shortcut (c2w, c2b; -1 when the identity).  M_NREF: the
+  // RCU convolutions of each input (adapt[i], 4 each) and of the output (outc, 2 per block), the MSF convolutions
+  // (msfw / msfb, one per input when there are two) and the CRP convolutions (crp).  M_NHEAD: normalizer in[0], end_conv (w, b).
+  int dil = 1;
+  int in[2][3] = {{-1, -1, -1}, {-1, -1, -1}};
+  int nin = 0;
+  std::vector<int> adapt[2], outc, msfw, msfb, crp;
 };
 
 struct Tensor {
@@ -182,7 +192,106 @@ bool has_attn(const b200_ncsnpp_config& c, int res) {
   return false;
 }
 
+// NCSNv2 walk (family 2): the level table of NCSNv2 (models/ncsnv2.py:43-100; num_levels = 4, the 'ncsnv2_64' network)
+// and NCSNv2_128 (:221-276; num_levels = 5).  Level l has two ResidualBlocks with chans[l] output channels and filter
+// dilation dil[l]; the first block of levels l > 0 is resample='down' (a 2x2 mean after its convolutions when dil[l] = 1,
+// no resampling when dilated).  refine k (k = 1..L) takes [layer L-k (, the previous refine output)] to feat[k-1] channels.
+struct NcsnWalk { int L; int chans[5]; int dil[5]; int feat[5]; };
+NcsnWalk ncsnv2_walk(int L, int nf) {
+  if (L == 4) return {4, {nf, 2 * nf, 2 * nf, 2 * nf}, {1, 1, 2, 4}, {2 * nf, 2 * nf, nf, nf}};
+  return {5, {nf, 2 * nf, 2 * nf, 4 * nf, 4 * nf}, {1, 1, 1, 2, 4}, {4 * nf, 2 * nf, 2 * nf, nf, nf}};
+}
+
+int build_graph_ncsnv2(b200_ncsnpp* e) {
+  const b200_ncsnpp_config& c = e->cfg;
+  const int nf = c.nf, ch = c.num_channels, R = c.image_size;
+  const NcsnWalk wk = ncsnv2_walk(c.num_levels, nf);
+  const bool tcmode = c.precision != 1;
+  const int om = c.precision == 2 ? 2 : 1;
+  // a 3x3 / 1x1 convolution weight OIHW -> [tap][O][I], packed in the operand format when it runs on the tensor cores
+  // (Param::round != 0 marks those; the walk reads it back)
+  auto conv_param = [&](const std::string& name, int cin, int cout, int taps, int res, int dil, bool bias, int* pb) {
+    TcGemmDesc d = tc_desc(e, nullptr, cin, nullptr, 0, res, res, 1, taps, nullptr, cout);
+    d.dilation = dil;
+    const bool tc = tcmode && tc_gemm_supported(d, nullptr);
+    const int k = taps == 9 ? 3 : 1;
+    const int pw = add_param(e, name + ".weight", {cout, cin, k, k}, PK_CONV, taps, cout, cin, tc ? om : 0);
+    if (pb) *pb = bias ? add_param(e, name + ".bias", {cout}, PK_COPY, 0, 0, 0, 0) : -1;
+    return pw;
+  };
+  auto in_params = [&](const std::string& name, int C, int (&dst)[3]) {   // InstanceNorm2dPlus: alpha, gamma, beta
+    for (int k = 0; k < 3; ++k) dst[k] = add_param(e, name + (k == 0 ? ".alpha" : k == 1 ? ".gamma" : ".beta"), {C}, PK_COPY, 0, 0, 0, 0);
+  };
+  // begin_conv (ncsnv2.py:55): the input convolution of the shared walk (im2col + one K=32 contraction on the tensor cores)
+  { Mod m; m.kind = M_CONV_IN; m.index = 0; m.cin1 = ch; m.cout = nf; m.res = R;
+    m.tc0 = tcmode && (9 * ch <= 32) && (nf % 128 == 0);
+    const int om_in = c.precision == 2 ? 2 : 1;
+    m.w = m.tc0 ? add_param(e, "begin_conv.weight", {nf, ch, 3, 3}, PK_CONV_FLAT32, 9, nf, ch, om_in, -1, (long long)nf * 32)
+                : add_param(e, "begin_conv.weight", {nf, ch, 3, 3}, PK_CONV, 9, nf, ch, 0);
+    m.b = add_param(e, "begin_conv.bias", {nf}, PK_COPY, 0, 0, 0, 0); e->mods.push_back(m); }
+  // normalizer and end_conv are registered right after begin_conv (ncsnv2.py:57-58) and run last
+  Mod head; head.kind = M_NHEAD; head.index = -1; head.cin1 = nf; head.cout = ch; head.res = R;
+  in_params("normalizer", nf, head.in[0]);
+  head.w = add_param(e, "end_conv.weight", {ch, nf, 3, 3}, PK_CONV, 9, ch, nf, 0);
+  head.b = add_param(e, "end_conv.bias", {ch}, PK_COPY, 0, 0, 0, 0);
+  // ResidualBlock (layers.py:453-507) in its registration order: conv1, normalize2, conv2, shortcut, normalize1
+  int res = R, cin = nf, idx = 1;
+  std::vector<int> level_res;
+  for (int l = 0; l < wk.L; ++l) {
+    for (int b = 0; b < 2; ++b) {
+      Mod m; m.kind = M_NRES; m.index = idx++; m.cin1 = cin; m.cout = wk.chans[l]; m.dil = wk.dil[l]; m.res = res;
+      m.down = (l > 0 && b == 0) ? 1 : 0;
+      const std::string nm = "res" + std::to_string(l + 1) + "." + std::to_string(b);
+      const int d = m.dil, mid = m.down ? cin : m.cout;
+      m.c0w = conv_param(nm + ".conv1", cin, mid, 9, res, d, true, &m.c0b);
+      in_params(nm + ".normalize2", mid, m.in[1]);
+      const bool meanpool = m.down && d == 1;   // ConvMeanPool (layers.py:351-369): the convolution at full resolution
+      m.c1w = conv_param(nm + (meanpool ? ".conv2.conv" : ".conv2"), mid, m.cout, 9, res, d, true, &m.c1b);
+      if (m.cout != cin || m.down) {
+        // ConvMeanPool with a 1x1 filter, ncsn_conv1x1, or the dilated 3x3 (conv_shortcut, layers.py:462-484)
+        const int taps = d > 1 ? 9 : 1;
+        m.c2w = conv_param(nm + (meanpool ? ".shortcut.conv" : ".shortcut"), cin, m.cout, taps, res, d, true, &m.c2b);
+      }
+      in_params(nm + ".normalize1", cin, m.in[0]);
+      e->mods.push_back(m);
+      if (meanpool) res /= 2;
+      cin = m.cout;
+    }
+    level_res.push_back(res);
+  }
+  // RefineBlock (layers.py:277-310) in its registration order: adapt_convs, output_convs, msf, crp
+  for (int k = 1; k <= wk.L; ++k) {
+    Mod m; m.kind = M_NREF; m.index = idx++;
+    const int lay = wk.L - k, F = wk.feat[k - 1];
+    const int ins[2] = {wk.chans[lay], k > 1 ? wk.feat[k - 2] : 0};
+    const int rin[2] = {level_res[lay], k > 1 ? level_res[lay + 1] : 0};
+    m.nin = k > 1 ? 2 : 1; m.cin1 = ins[0]; m.cout = F; m.res = level_res[lay];
+    const bool end = k == wk.L;   // the output RCU has three blocks
+    const std::string nm = "refine" + std::to_string(k);
+    for (int i = 0; i < m.nin; ++i)
+      for (int bl = 1; bl <= 2; ++bl)
+        for (int st = 1; st <= 2; ++st)
+          m.adapt[i].push_back(conv_param(nm + ".adapt_convs." + std::to_string(i) + "." + std::to_string(bl) + "_" +
+                                          std::to_string(st) + "_conv", ins[i], ins[i], 9, rin[i], 1, false, nullptr));
+    for (int bl = 1; bl <= (end ? 3 : 1); ++bl)
+      for (int st = 1; st <= 2; ++st)
+        m.outc.push_back(conv_param(nm + ".output_convs." + std::to_string(bl) + "_" + std::to_string(st) + "_conv", F, F, 9,
+                                    m.res, 1, false, nullptr));
+    if (m.nin > 1)
+      for (int i = 0; i < 2; ++i) {
+        int pb = -1;
+        m.msfw.push_back(conv_param(nm + ".msf.convs." + std::to_string(i), ins[i], F, 9, rin[i], 1, true, &pb));
+        m.msfb.push_back(pb);
+      }
+    for (int i = 0; i < 2; ++i) m.crp.push_back(conv_param(nm + ".crp.convs." + std::to_string(i), F, F, 9, m.res, 1, false, nullptr));
+    e->mods.push_back(m);
+  }
+  e->mods.push_back(head);
+  return 0;
+}
+
 int build_graph(b200_ncsnpp* e) {
+  if (e->cfg.family == 2) return build_graph_ncsnv2(e);
   const b200_ncsnpp_config& c = e->cfg;
   const bool ddpm = c.family == 1;
   B200_REQUIRE(c.num_levels >= 1 && c.num_levels <= 8, "ncsnpp: num_levels=%d out of range", c.num_levels);
@@ -440,6 +549,8 @@ struct Conv {
   // fused skip projection: the 1x1 conv (weights pw, bias pb) of x1 (+ x2) as extra K steps (tensor-core path)
   Conv& skip(const Tensor& x1, const Tensor& x2, int pw, int pb) { skip1_ = x1; skip2_ = x2; skip_w_ = pw; skip_b_ = pb; return *this; }
   Conv& gn(const Coef& c) { gn_ = &c; return *this; }                   // GroupNorm+SiLU on load (few-channel kernel)
+  int dil_ = 1;
+  Conv& dilation(int d) { dil_ = d; return *this; }                     // 3x3 'same' filter taps d pixels apart (padding d)
 };
 
 struct Builder {
@@ -462,7 +573,7 @@ struct Builder {
     char buf[160]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof(buf), fmt, ap); va_end(ap); next_name = buf;
   }
   Builder(b200_ncsnpp* e_, int B_, char* base_, bool dry_, int lane_ = 0) : e(e_), B(B_), base(base_), dry(dry_), arena(e_->cfg.keep_activations != 0), lane(lane_) {
-    fused_stats = e_->cfg.precision != 1;
+    fused_stats = e_->cfg.precision != 1 && e_->cfg.family != 2;   // (NCSNv2's InstanceNorm statistics take a pass of their own)
     split = e_->cfg.precision == 3;
     om = e_->cfg.precision == 2 ? 2 : split ? 0 : 1;
     tan = e_->cfg.tangent != 0;
@@ -672,6 +783,7 @@ struct Builder {
     if (use_tc) {
       TcGemmDesc d = tc_desc(e, a1.p, a1.C, a2.p, a2.C, out.H, out.W, B, taps, e->W(pw), Cout);
       d.stride = stride; d.valid_pad = stride == 2 ? 1 : 0; d.Hin = Hin ? Hin : out.H; d.Win = Hin ? Hin : out.W;
+      d.dilation = o.dil_;
       if (dense_row >= 0) ep.rowvec = dense_all + dense_row;
       if (x3.p) {   // fused skip projection: its bias rides in the (image-independent) row-vector slot
         if (dense_row >= 0) { set_error("ncsnpp: fused skip projection on a conv with a time-embedding bias"); rc = 2; return; }
@@ -700,6 +812,7 @@ struct Builder {
       e->tcplans.push_back(pl);
       name("conv%s %d+%d->%d @%d%s%s%s [%s]", taps == 9 ? "3x3" : "1x1", a1.C, a2.C, Cout, out.H, stride == 2 ? " s2" : "",
            x3.p ? " +skipproj" : "", residual ? " +res" : "", tc_gemm_form(pl));
+      if (o.dil_ > 1) next_name += " d" + std::to_string(o.dil_);
       if (x3.p) next_name += " " + std::to_string(x3.C + x4.C);
       {
         const double es = om == 2 ? 2.0 : split ? 8.0 : 4.0, px = (double)B * out.H * out.W;   // split TF32: hi + lo
@@ -714,6 +827,7 @@ struct Builder {
     } else {
       SimtConv s = simt_desc(a1.p, a1.C, a1.H, a1.W, taps, 1, a1.H, a1.W, e->W(pw), Cout);
       s.x2 = a2.p; s.C2 = a2.C;
+      if (o.dil_ > 1) { s.dilation = o.dil_; s.pad = o.dil_; }
       if (dense_row >= 0) ep.rowvec = dense_all + dense_row;
       s.epi = ep;
       // few-channel levels of the nf = 16 networks: warp-level TF32 MMAs keep them at the HBM roofline (conv_lowc.cu);
@@ -726,6 +840,7 @@ struct Builder {
         s.gn_scale = o.gn_->scale; s.gn_shift = o.gn_->shift; s.gn_act = 1;
       }
       name("conv%s %s%d+%d->%d @%d [%s]", taps == 9 ? "3x3" : "1x1", o.gn_ ? "gn+silu " : "", a1.C, a2.C, Cout, out.H, lowc ? "mma.sync tf32" : "cuda-core");
+      if (o.dil_ > 1) next_name += " d" + std::to_string(o.dil_);
       next_bytes = (double)B * out.H * out.W * ((a1.C + a2.C) * 4.0 + Cout * 4.0 + (residual ? Cout * 4.0 : 0.0)) +
                    (double)taps * (a1.C + a2.C) * Cout * 4.0;
       op(1, [=](cudaStream_t st) {
@@ -1263,8 +1378,211 @@ struct Builder {
     tfree(a);
   }
 
+  // ===== NCSNv2 (family 2) =====
+  // would the contraction with packed weight pi run on the tensor cores (its weights are packed in the operand format)?
+  bool on_tc(int pi) const { return pi >= 0 && e->params[pi].round != 0; }
+  int mode_for(int pi) const { return on_tc(pi) ? om : 0; }
+  // InstanceNorm2dPlus (normalization.py:157-183) of x with parameters p = {alpha, gamma, beta}, then ELU, into y in
+  // store mode `mode`: one fp64 statistics pass and one apply pass
+  void in_elu(const Tensor& x, const int (&p)[3], int mode, const Tensor& y) {
+    long long sb; double* stats = reinterpret_cast<double*>(falloc(2 * in_stats_doubles(B, x.H * x.W, x.C), &sb));   // (floats)
+    const Tensor xx = x; const int Bc = B, HW = x.H * x.W;
+    const float *al = e->W(p[0]), *ga = e->W(p[1]), *be = e->W(p[2]);
+    name("in++ stats %d @%d", x.C, x.H);
+    next_bytes = (double)B * HW * x.C * 4.0;
+    const int nl = in_stats_doubles(B, HW, x.C) > 2LL * B * x.C ? 2 : 1;   // pixel slices + their reduction
+    op(nl, [=](cudaStream_t st) { return launch_in_stats(xx.p, Bc, HW, xx.C, stats, st); }, 2);
+    name("in++ apply elu %d @%d%s", x.C, x.H, mode == 2 ? " f16-out" : "");
+    next_bytes = (double)B * HW * x.C * (4.0 + (mode == 2 ? 2.0 : 4.0));
+    op(1, [=](cudaStream_t st) { return launch_in_apply(xx.p, stats, al, ga, be, Bc, HW, xx.C, 1e-5f, 1, mode, y.p, st); }, 2);
+    ffree(reinterpret_cast<float*>(stats), sb);
+  }
+  Tensor elu(const Tensor& x, int mode) {
+    Tensor y = talloc(x.C, x.H, x.W);
+    const long long n = (long long)B * x.H * x.W * x.C;
+    const float* src = x.p;
+    name("elu %d @%d%s", x.C, x.H, mode == 2 ? " f16-out" : "");
+    next_bytes = n * (4.0 + (mode == 2 ? 2.0 : 4.0));
+    op(1, [=](cudaStream_t st) { return launch_elu_operand(src, y.p, n, mode, st); }, 6);
+    return y;
+  }
+  // x itself when the contraction reads fp32 (CUDA cores), else a copy in the operand format
+  Tensor operand(const Tensor& x, bool tc, bool* owned) {
+    *owned = tc;
+    if (!tc) return x;
+    Tensor y = talloc(x.C, x.H, x.W);
+    const long long n = (long long)B * x.H * x.W * x.C; const int omc = om; const float* src = x.p;
+    name("operand copy %d @%d", x.C, x.H);
+    next_bytes = (double)n * (4.0 + (om == 2 ? 2.0 : 4.0));
+    op(1, [=](cudaStream_t st) { return launch_store_operand(src, y.p, n, omc, st); }, 6);
+    return y;
+  }
+
+  // ResidualBlock (layers.py:453-507): normalize1, ELU, conv1, normalize2, ELU, conv2, + shortcut.  conv2 adds the shortcut
+  // (the identity, a 1x1 / dilated 3x3 convolution of x) in its epilogue; a resample='down' block at dilation 1
+  // (ConvMeanPool, layers.py:351-369) then takes the 2x2 mean of that sum.
+  Tensor nres(const Mod& m, const Tensor& x) {
+    Tensor none;
+    const int H = x.H, mid = m.down ? m.cin1 : m.cout, d = m.dil;
+    const bool meanpool = m.down && d == 1;
+    Tensor a = talloc(m.cin1, H, H);
+    in_elu(x, m.in[0], mode_for(m.c0w), a);
+    Tensor t = talloc(mid, H, H);
+    conv(on_tc(m.c0w), a, none, m.c0w, m.c0b, t, Conv().dilation(d));
+    tfree(a);
+    Tensor a2 = talloc(mid, H, H);
+    in_elu(t, m.in[1], mode_for(m.c1w), a2);
+    tfree(t);
+    Tensor sc;
+    if (m.c2w >= 0) {
+      bool owned; Tensor xo = operand(x, on_tc(m.c2w), &owned);
+      sc = talloc(m.cout, H, H);
+      conv(on_tc(m.c2w), xo, none, m.c2w, m.c2b, sc, Conv().taps(d > 1 ? 9 : 1).dilation(d));
+      if (owned) tfree(xo);
+    }
+    Tensor full = talloc(m.cout, H, H);
+    conv(on_tc(m.c1w), a2, none, m.c1w, m.c1b, full, Conv().dilation(d).residual(sc.p ? sc : x));
+    tfree(a2); tfree(sc);
+    if (!meanpool) return full;
+    Tensor out = talloc(m.cout, H / 2, H / 2);
+    fir(full.p, B, H, H, m.cout, 1, 2, 0, 0, 0, out.p, 0.25f, /*box=*/true);   // mean of each 2x2 cell
+    tfree(full);
+    return out;
+  }
+
+  // RCUBlock(features, n_blocks, 2) (layers.py:183-204): per block x = conv(ELU(conv(ELU(x)))) + x, 3x3 without bias.
+  // The last block's output is stored in mode `out_mode` (the operand of an MSF convolution), the rest fp32.  x stays owned by
+  // the caller.
+  Tensor rcu(const Tensor& x, const std::vector<int>& convs, int out_mode) {
+    Tensor none, cur = x;
+    const int nblk = (int)convs.size() / 2;
+    for (int k = 0; k < nblk; ++k) {
+      const int c1 = convs[2 * k], c2 = convs[2 * k + 1];
+      Tensor e1 = elu(cur, mode_for(c1));
+      Tensor t = talloc(x.C, x.H, x.W);
+      conv(on_tc(c1), e1, none, c1, -1, t);
+      tfree(e1);
+      Tensor e2 = elu(t, mode_for(c2));
+      tfree(t);
+      Tensor nx = talloc(x.C, x.H, x.W);
+      conv(on_tc(c2), e2, none, c2, -1, nx, Conv().residual(cur).round(k == nblk - 1 ? out_mode : 0));
+      tfree(e2);
+      if (k > 0) tfree(cur);
+      cur = nx;
+    }
+    return cur;
+  }
+
+  // RefineBlock (layers.py:277-310): adapt RCUs, MSF (layers.py:236-250: a 3x3 conv with bias of each input, bilinearly
+  // resized to the first input's size, summed into zeros in input order), CRP (layers.py:133-154, max pooling), output RCU
+  Tensor refine(const Mod& m, const Tensor* xs) {
+    Tensor none, h;
+    Tensor hs[2];
+    for (int i = 0; i < m.nin; ++i) {
+      // an MSF input is only read by its MSF convolution: the RCU's last epilogue writes it in that operand format
+      const int msf_tc = m.nin > 1 && on_tc(m.msfw[i]) && on_tc(m.adapt[i][3]);
+      hs[i] = rcu(xs[i], m.adapt[i], msf_tc ? om : 0);
+      if (m.nin > 1 && on_tc(m.msfw[i]) && !msf_tc) {   // CUDA-core RCU feeding a tensor-core MSF convolution
+        bool owned; Tensor o = operand(hs[i], true, &owned);
+        tfree(hs[i]); hs[i] = o;
+      }
+    }
+    if (m.nin > 1) {
+      const int F = m.cout, Ho = hs[0].H;
+      Tensor h0 = talloc(F, Ho, Ho);
+      conv(on_tc(m.msfw[0]), hs[0], none, m.msfw[0], m.msfb[0], h0);
+      tfree(hs[0]);
+      if (hs[1].H == Ho) {   // same size: the interpolation is the identity, 0 + h0 + h1 = conv1 + bias + h0 in the epilogue
+        h = talloc(F, Ho, Ho);
+        conv(on_tc(m.msfw[1]), hs[1], none, m.msfw[1], m.msfb[1], h, Conv().residual(h0));
+        tfree(h0);
+      } else {
+        Tensor h1 = talloc(F, hs[1].H, hs[1].W);
+        conv(on_tc(m.msfw[1]), hs[1], none, m.msfw[1], m.msfb[1], h1);
+        const int Bc = B, Hl = h1.H, Fc = F;
+        name("bilinear 2x +sum %d @%d", F, Ho);
+        next_bytes = (double)B * F * (Hl * Hl + 2.0 * Ho * Ho) * 4.0;
+        op(1, [=](cudaStream_t st) { return launch_bilinear_add(h1.p, Bc, Hl, Hl, Fc, h0.p, Ho, Ho, st); }, 3);
+        tfree(h1);
+        h = h0;
+      }
+      tfree(hs[1]);
+    } else {
+      h = hs[0];
+    }
+    // CRP: x = ELU(x); path = x; twice: path = conv(maxpool(path)); x = path + x.  The second pool also writes
+    // x1 = path1 + ELU(x), which the last convolution adds in its epilogue.
+    const int F = h.C, H = h.H, Bc = B;
+    Tensor xa = elu(h, 0);
+    tfree(h);
+    Tensor pool0 = talloc(F, H, H);
+    { const int md = mode_for(m.crp[0]); name("maxpool5x5 %d @%d", F, H); next_bytes = (double)B * H * H * F * 8.0;
+      op(1, [=](cudaStream_t st) { return launch_maxpool5(xa.p, Bc, H, H, F, md, pool0.p, nullptr, nullptr, st); }, 6); }
+    Tensor path1 = talloc(F, H, H);
+    conv(on_tc(m.crp[0]), pool0, none, m.crp[0], -1, path1);
+    tfree(pool0);
+    Tensor pool1 = talloc(F, H, H), x1 = talloc(F, H, H);
+    { const int md = mode_for(m.crp[1]); name("maxpool5x5 +sum %d @%d", F, H); next_bytes = (double)B * H * H * F * 16.0;
+      op(1, [=](cudaStream_t st) { return launch_maxpool5(path1.p, Bc, H, H, F, md, pool1.p, xa.p, x1.p, st); }, 6); }
+    tfree(path1); tfree(xa);
+    Tensor x2 = talloc(F, H, H);
+    conv(on_tc(m.crp[1]), pool1, none, m.crp[1], -1, x2, Conv().residual(x1));
+    tfree(pool1); tfree(x1);
+    Tensor out = rcu(x2, m.outc, 0);
+    tfree(x2);
+    return out;
+  }
+
+  // output (ncsnv2.py:124-132): normalizer, ELU, end_conv, / sigmas[y] (the caller passes sigma per image as the label)
+  void nhead(const Mod& m, Tensor& h) {
+    const int R = h.H, ch = m.cout, ln = lane, Bc = B, C = h.C;
+    b200_ncsnpp* eng = e;
+    Tensor a = talloc(C, R, R);
+    in_elu(h, m.in[0], 0, a);
+    tfree(h);
+    const float *wo = e->W(m.w), *bo = e->W(m.b);
+    name("conv3x3 %d->%d @%d nchw-out /sigma [small-n]", C, ch, R);
+    next_bytes = (double)B * R * R * (C + ch) * 4.0;
+    op(1, [=](cudaStream_t st) {
+      return launch_conv3x3_small_n(a.p, wo, bo, eng->in_labels_l[ln], eng->uniform ? 0 : 1, eng->out_l[ln], Bc, R, R, C, ch, 0, st);
+    }, 1, 2.0 * B * R * R * (double)ch * C * 9);
+    tfree(a);
+  }
+
+  // the forward pass of NCSNv2 / NCSNv2_128 (ncsnv2.py:107-132, 278-312) as a walk over e->mods
+  int build_ncsnv2() {
+    mi = 0;
+    const int L = e->cfg.num_levels;
+    Tensor x = input_conv();   // 2x - 1 (unless centred), begin_conv
+    if (rc) return rc;
+    std::vector<Tensor> layers;
+    for (int l = 0; l < L; ++l) {
+      const Mod& m0 = next(); Tensor a = nres(m0, x); if (rc) return rc;
+      tap(m0.index, a);
+      if (l == 0) tfree(x);   // begin_conv's output; later levels keep their input in `layers`
+      const Mod& m1 = next(); Tensor b = nres(m1, a); if (rc) return rc;
+      tap(m1.index, b);
+      tfree(a);
+      layers.push_back(b); x = b;
+    }
+    Tensor ref;
+    for (int k = 1; k <= L; ++k) {
+      const Mod& m = next();
+      const Tensor xs[2] = {layers[L - k], ref};
+      Tensor r = refine(m, xs); if (rc) return rc;
+      tap(m.index, r);
+      tfree(layers[L - k]); tfree(ref);
+      ref = r;
+    }
+    const Mod& mh = next();
+    nhead(mh, ref);
+    if (mi != e->mods.size()) { set_error("ncsnv2: plan walked %zu of %zu modules", mi, e->mods.size()); return 2; }
+    return rc;
+  }
+
   // the forward pass (models/ncsnpp.py:232-381) as a walk over e->mods
   int build() {
+    if (e->cfg.family == 2) return build_ncsnv2();
     const b200_ncsnpp_config& c = e->cfg;
     const int L = c.num_levels;
     Tensor none;
@@ -1339,7 +1657,7 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
   B200_REQUIRE(cfg && out, "ncsnpp_create: null argument");
   B200_REQUIRE(cfg->no_halo == 0 || cfg->no_halo == 1, "ncsnpp_create: no_halo=%d unknown (0 halo form, 1 one tile per tap)",
                cfg->no_halo);
-  B200_REQUIRE(cfg->family == 0 || cfg->family == 1, "ncsnpp_create: family=%d unknown (0 NCSN++, 1 DDPM)", cfg->family);
+  B200_REQUIRE(cfg->family >= 0 && cfg->family <= 2, "ncsnpp_create: family=%d unknown (0 NCSN++, 1 DDPM, 2 NCSNv2)", cfg->family);
   B200_REQUIRE(cfg->precision >= 0 && cfg->precision <= 3, "ncsnpp_create: precision=%d unknown (0 tf32, 1 fp32, 2 f16, 3 split tf32)",
                cfg->precision);
   if (cfg->family == 1) {
@@ -1347,6 +1665,19 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
                  "without time conditioning, models/ddpm.py:58-71)");
     B200_REQUIRE(!cfg->scale_by_sigma, "ncsnpp_create: DDPM (family 1) with scale_by_sigma = 1 (configs/ve/cifar10_ddpm.py) is not "
                  "supported by the engine");
+  }
+  if (cfg->family == 2) {
+    B200_REQUIRE(!cfg->tangent, "ncsnpp_create: family = 2 (NCSNv2) has no forward-mode tangent pass (tangent = 1)");
+    B200_REQUIRE(cfg->precision != 3, "ncsnpp_create: family = 2 (NCSNv2) runs in precision 0 (tf32), 1 (fp32) or 2 (f16), not "
+                 "3 (split tf32)");
+    B200_REQUIRE(cfg->num_levels == 4 || cfg->num_levels == 5, "ncsnpp_create: family = 2 (NCSNv2) has num_levels = 4 (ncsnv2_64) "
+                 "or 5 (ncsnv2_128), got %d", cfg->num_levels);
+    B200_REQUIRE(cfg->nf >= 4 && cfg->nf % 4 == 0 && cfg->nf * (cfg->num_levels == 5 ? 4 : 2) <= 512,
+                 "ncsnpp_create: family = 2 (NCSNv2) needs nf a multiple of 4 with at most 512 channels per level, got nf=%d", cfg->nf);
+    B200_REQUIRE(cfg->num_channels >= 1 && cfg->num_channels <= 4, "ncsnpp_create: family = 2 (NCSNv2) takes 1..4 image channels, "
+                 "got %d", cfg->num_channels);
+    B200_REQUIRE(cfg->image_size >= 8 && cfg->image_size % (cfg->num_levels == 5 ? 8 : 4) == 0,
+                 "ncsnpp_create: family = 2 (NCSNv2): image_size=%d does not halve %d times", cfg->image_size, cfg->num_levels == 5 ? 3 : 2);
   }
   if (cfg->tangent) {
     // the forward-mode tangent pass (b200_ncsnpp_jvp) covers DDPM and the DDPM++ family; everything else is refused here
@@ -1371,6 +1702,13 @@ int b200_ncsnpp_create(const b200_ncsnpp_config* cfg, b200_ncsnpp_t** out) {
     b200_ncsnpp_config& c = e->cfg;
     c.skip_rescale = 0; c.progressive_input = 0; c.progressive = 0; c.embedding_type = 1; c.naive_resample = 1;
     c.fir_taps = 1; c.fir_kernel[0] = 1.f;
+  }
+  if (cfg->family == 2) {
+    // NCSNv2 reads image_size, num_channels, nf, num_levels, centered and the execution fields; the rest takes the values
+    // that keep the shared paths inert: no pyramids, no time embedding, a unit FIR no layer reads
+    b200_ncsnpp_config& c = e->cfg;
+    c.skip_rescale = 0; c.progressive_input = 0; c.progressive = 0; c.embedding_type = 0; c.naive_resample = 1;
+    c.fir_taps = 1; c.fir_kernel[0] = 1.f; c.scale_by_sigma = 1; c.conditional = 1; c.num_res_blocks = 2;
   }
   if (int r = build_graph(e)) { delete e; return r; }
   *out = e;

@@ -50,6 +50,7 @@ struct TcParams {
   int halo_copy_bytes;                     // (tile rows + 2) * W * 128: bytes of one halo copy
   int chunk_major;                         // nine-load loop walks K as (chunk, filter column, filter row): shapes with a halo form
   int conv, H, W, taps, pad, S, stride;   // H, W: OUTPUT spatial size; S = filter width (3 or 1)
+  int dil;                                 // filter tap spacing (1 dense; 2 / 4: the NCSNv2 dilated blocks, nine-load form only)
   int kchunks[4];                          // channel chunks of each source (0: no such source)
   int wcol[4];                             // first weight column of each source: 0, C1 in w[0]; 0, C3 in w[1]
   int N_total, tiles_n;
@@ -343,7 +344,7 @@ __device__ __forceinline__ void produce_taps(const TcParams& p, uint8_t* smem, u
         for (int i = 0; i < ninner; ++i) {
           const int kc = p.chunk_major ? o : i, t = p.chunk_major ? i : o;
           const int tap = (ntaps == 1 || !p.chunk_major) ? t : (t % p.S) * p.S + t / p.S;
-          const int dh = src < 2 ? tap / p.S - p.pad : 0, dw = src < 2 ? tap % p.S - p.pad : 0;
+          const int dh = src < 2 ? (tap / p.S - p.pad) * p.dil : 0, dw = src < 2 ? (tap % p.S - p.pad) * p.dil : 0;
           for (int ph = 0; ph < p.nphase; ++ph) {
             const PhaseMaps m = phase_maps(p, p.a[src], p.w[src >> 1], ph);
             mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -699,6 +700,9 @@ bool tc_gemm_supported(const TcGemmDesc& d, const char** why) {
     if (d.nbatch != 1) return fail("conv mode is unbatched");
     if (d.stride > 2) return fail("stride must be 1 or 2");
     if (d.stride == 2 && d.a2) return fail("strided conv is single-source");
+    if (d.dilation > 1 && (d.taps != 9 || d.stride == 2 || d.valid_pad || (d.Hin && d.Hin != d.H) || (d.Win && d.Win != d.W)))
+      return fail("dilated filters are 3x3 'same' stride-1 convolutions");
+    if (d.dilation > 1 && (d.a3 || d.split)) return fail("dilated filters take no extra 1x1 phase and no split TF32 operands");
     const int HW = d.H * d.W;
     if (HW >= BM) {
       if (d.W >= BM) { if (d.W % BM) return fail("image width does not tile 128 pixels"); }
@@ -731,10 +735,10 @@ bool tc_gemm_supported(const TcGemmDesc& d, const char** why) {
   return true;
 }
 
-// 'same'-padded stride-1 3x3 filters on 16- or 32-pixel-wide images, read at their output size: the shapes that have a
-// halo form.
+// 'same'-padded stride-1 dense 3x3 filters on 16- or 32-pixel-wide images, read at their output size: the shapes that have
+// a halo form (its copies carry a one-pixel halo, so dilated filters take the nine-load form).
 static bool has_halo_shape(const TcGemmDesc& d) {
-  return d.conv && d.taps == 9 && !d.valid_pad && d.stride != 2 && (d.W == 16 || d.W == 32) && (d.Hin == 0 || d.Hin == d.H) &&
+  return d.conv && d.taps == 9 && d.dilation <= 1 && !d.valid_pad && d.stride != 2 && (d.W == 16 || d.W == 32) && (d.Hin == 0 || d.Hin == d.H) &&
          (d.Win == 0 || d.Win == d.W);
 }
 
@@ -791,6 +795,7 @@ int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out) {
   p.conv = d.conv; p.H = d.conv ? d.H : 1; p.W = d.conv ? d.W : 1; p.taps = d.taps;
   p.S = d.taps == 9 ? 3 : 1; p.pad = (d.taps == 9 && !d.valid_pad) ? 1 : 0;
   p.stride = d.stride == 2 ? 2 : 1;
+  p.dil = d.dilation > 1 ? d.dilation : 1;
   p.f16 = d.f16 ? 1 : 0;
   p.nphase = d.split ? 3 : 1;
   p.swap = form.swap; p.halo = form.halo; p.chunk_major = form.chunk_major;

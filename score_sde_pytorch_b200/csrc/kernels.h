@@ -84,6 +84,7 @@ struct SimtConv {
   // (sum, sum of squares), zeroed by the caller; null = none
   double* qstats;
   Epilogue epi;
+  int dilation;                     // filter taps dilation apart (0 or 1: dense); 'same' convolutions then pad by dilation
 };
 int launch_conv_simt(const SimtConv& p, cudaStream_t st);
 
@@ -131,6 +132,9 @@ struct TcGemmDesc {
   // lo_A hi_W + hi_A lo_W + hi_A hi_W (small terms first).  TF32 operands only.
   int split;
   const float *a1_lo, *a2_lo, *a3_lo, *a4_lo, *w_lo, *w2_lo;
+  // conv, 3x3 'same' stride 1: filter tap (r, s) reads pixel (y + dilation (r - 1), x + dilation (s - 1)), TMA's
+  // out-of-bounds fill being the zero padding (0 or 1: dense).  Dilated filters run the nine-load mainloop only.
+  int dilation;
 };
 int tc_gemm_plan_create(const TcGemmDesc& d, TcGemmPlan** out);
 void tc_gemm_plan_destroy(TcGemmPlan* p);
@@ -174,6 +178,22 @@ struct AttnFlashPlan {
 bool attn_flash_supported(int T, int C);
 int attn_flash_plan(const void* qk, const void* vT, const float* bv, void* out, int nimg, int T, int C, AttnFlashPlan* pl);
 int attn_flash_launch(const AttnFlashPlan& p, cudaStream_t st);
+
+// ---- ncsnv2.cu : InstanceNorm2dPlus, ELU, the CRP max pool and the MSF bilinear sum (NHWC fp32 activations) ----------
+// stats [B][C][2] fp64 (sum, sum of squares over HW), written (not accumulated; no zeroing needed), in a buffer of
+// in_stats_doubles(B, HW, C) doubles: large images are summed in up to IN_MAX_SLICES pixel slices, whose partials follow
+// the [B][C][2] sums and are added in slice order
+constexpr int IN_MAX_SLICES = 32;
+long long in_stats_doubles(int B, int HW, int C);
+int launch_in_stats(const float* x, int B, int HW, int C, double* stats, cudaStream_t st);
+// y = act ? ELU(IN++(x)) : IN++(x) in operand format `mode` (0 fp32, 1 TF32 grid, 2 fp16); C % 4 == 0, C <= 512
+int launch_in_apply(const float* x, const double* stats, const float* alpha, const float* gamma, const float* beta, int B,
+                    int HW, int C, float eps, int act, int mode, float* y, cudaStream_t st);
+int launch_elu_operand(const float* x, float* y, long long n, int mode, cudaStream_t st);
+// y = maxpool5x5_s1_p2(x) in operand format `mode`; with add: sum = x + add (fp32)
+int launch_maxpool5(const float* x, int B, int H, int W, int C, int mode, float* y, const float* add, float* sum, cudaStream_t st);
+// acc += bilinear upsample (align_corners=True) of lo [B][Hl][Wl][C] to H x W
+int launch_bilinear_add(const float* lo, int B, int Hl, int Wl, int C, float* acc, int H, int W, cudaStream_t st);
 
 // ---- pc_update.cu -----------------------------------------------------------
 struct PhiloxMap {          // torch.randn_like's launch geometry for `numel` elements

@@ -41,6 +41,9 @@ def _engine_net(model):
   from . import native
   from .models._engine import EngineModel
   net = native._unwrap(model)
+  if isinstance(net, EngineModel) and not net.takes_time_labels:
+    raise NotImplementedError(f'likelihood: {type(net).__name__} takes noise-level indices, not the continuous-time labels '
+                              'of the probability-flow ODE')
   return net if isinstance(net, EngineModel) else None
 
 

@@ -32,6 +32,7 @@ class EngineModel(nn.Module):
   activations between layers), ``'tf32x3'`` (split TF32: every operand as a hi + lo pair of TF32 values, three wgmma
   products per K step into an fp32 accumulator - close to fp32 accuracy at tensor-core rate) or ``'fp32'`` (strict fp32
   on CUDA cores; validation mode)."""
+  takes_time_labels = True   # the label is a time / sigma value (False: integer noise-level indices, NCSNv2)
 
   def _set_engine_options(self, config, precision=None, keep_activations=False, lanes=1, cuda_core_head=None, pdl=None,
                           halo=None):
@@ -73,6 +74,12 @@ class EngineModel(nn.Module):
       c.attn_resolutions[i] = int(v)
     c.centered, c.scale_by_sigma = int(bool(cfg.data.centered)), int(bool(m.scale_by_sigma))
     c.conditional = int(bool(m.conditional))
+    self._execution_config(c)
+    self._family_config(c)
+    return c
+
+  def _execution_config(self, c):
+    """The execution fields of a ``b200_ncsnpp_config``, shared by every family."""
     c.pdl = int(self.pdl)
     c.no_halo = int(not self.halo)
     if self.precision not in ('tf32', 'fp32', 'f16', 'tf32x3'):
@@ -81,8 +88,6 @@ class EngineModel(nn.Module):
     c.keep_activations = int(self.keep_activations)
     c.lanes = self.lanes
     c.cuda_core_head = int(self.cuda_core_head)
-    self._family_config(c)
-    return c
 
   def native_param_table(self):
     """[(name, shape)] the engine expects, in its load order (no GPU needed)."""

@@ -292,6 +292,8 @@ def match_pc_plan(sde, model, predictor, corrector, shape, snr, n_steps, probabi
   model = _unwrap(model)
   if not isinstance(model, EngineModel) or torch.device(device).type != 'cuda' or not torch.cuda.is_available():
     return None
+  if not model.takes_time_labels:   # NCSNv2 evaluates noise-level indices: the host loop calls its forward
+    return None
   if type(sde) not in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE) or not continuous:
     return None
   pk, ck = _kind_of_predictor(predictor), _kind_of_corrector(corrector)

@@ -329,7 +329,11 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
     if not x.is_cuda:
       return False
     from .models._engine import EngineModel
-    ok = isinstance(native._unwrap(model), EngineModel) and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
+    net = native._unwrap(model)
+    ok = isinstance(net, EngineModel) and type(sde) in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE)
+    if ok and not net.takes_time_labels:
+      raise NotImplementedError(f'get_ode_sampler: {type(net).__name__} takes noise-level indices, not the continuous-time '
+                                'labels of the probability-flow ODE')
     if device_solver and not ok:
       raise NotImplementedError('get_ode_sampler(device_solver=True) needs an engine-backed network (NCSNpp or DDPM) and a '
                                 'VE/VP/sub-VP SDE')

@@ -18,7 +18,8 @@ ap.add_argument('--batch', type=int, default=1024)
 ap.add_argument('--precision', default='f16')
 ap.add_argument('--reps', type=int, default=5)
 ap.add_argument('--md', default=None)
-ap.add_argument('--config', default='headline', choices=['headline', 'celebahq_256', 'ddpmpp_256', 'ffhq_1024', 'cifar10_ddpmpp'])
+ap.add_argument('--config', default='headline', choices=['headline', 'celebahq_256', 'ddpmpp_256', 'ffhq_1024', 'cifar10_ddpmpp',
+                                                        'cifar10_ncsnv2'])
 ap.add_argument('--no-halo', action='store_true', help='3x3 mainloop with one shifted tile load per filter tap everywhere')
 args = ap.parse_args()
 dev = torch.device('cuda:0')
@@ -26,9 +27,13 @@ torch.manual_seed(0)
 from score_sde_pytorch_b200 import configs                          # noqa: E402
 cfg = {'headline': headline_config, 'celebahq_256': configs.ve_celebahq_256_ncsnpp_continuous,
        'ddpmpp_256': configs.subvp_celebahq_256_ddpmpp_continuous, 'ffhq_1024': configs.ve_ffhq_1024_ncsnpp_continuous,
-       'cifar10_ddpmpp': configs.vp_cifar10_ddpmpp_continuous}[args.config]()
-cfg.model.init_scale = 1.0
-model = NCSNpp(cfg, precision=args.precision, halo=not args.no_halo).to(dev)
+       'cifar10_ddpmpp': configs.vp_cifar10_ddpmpp_continuous, 'cifar10_ncsnv2': configs.ve_cifar10_ncsnv2}[args.config]()
+if args.config == 'cifar10_ncsnv2':   # configs/ve/ncsnv2/cifar10.py; the engine's label is the sigma the output is divided by
+  from score_sde_pytorch_b200.models.ncsnv2 import NCSNv2   # noqa: E402
+  model = NCSNv2(cfg, precision=args.precision, halo=not args.no_halo).to(dev)
+else:
+  cfg.model.init_scale = 1.0
+  model = NCSNpp(cfg, precision=args.precision, halo=not args.no_halo).to(dev)
 B = args.batch
 eng = model.engine(B, dev)
 h = eng['h']
