@@ -261,7 +261,7 @@ typedef struct {
                                 * Langevin dynamics (:286-319), whose step size depends on the step only: x_mean = ca x + cb out,
                                 * x = x_mean + cc z */
   int predictor;               /* 0 none, 1 affine (reverse_diffusion / euler_maruyama / ancestral_sampling: x_mean = pa x + pb out,
-                                * x = x_mean + pc z) */
+                                * x = x_mean + pc z), 2 multistep ODE update (mq, mr, pm1, pm2 below) */
   int n_corrector_steps;       /* config.sampling.n_steps_each */
   float snr;
   const float *label, *score_scale, *alpha, *pa, *pb, *pc;   /* HOST tables [n_steps] */
@@ -276,6 +276,13 @@ typedef struct {
   int noise_nhwc;              /* 1: every randn_like draw fills the state in channels-last memory order, as torch does for
                                 * a channels-last x (the reference's colorization state is its einsum's channels-last
                                 * output for batches > 1); 0: NCHW order */
+  /* predictor == 2: multistep exponential integrator of the probability-flow ODE (DPM-Solver / DPM-Solver++, orders 1-3),
+   * with corrector == 0 and constraint == 0.  Step i, after one network evaluation out_i = net(x_i, label[i]):
+   *   M_i     = mq[i] x_i + mr[i] out_i                                  (the data or noise prediction)
+   *   x_{i+1} = pa[i] x_i + pb[i] M_i + pm1[i] M_{i-1} + pm2[i] M_{i-2}
+   * each product and sum rounded separately in this order (a term whose coefficient is 0 is skipped), and x_mean = x.
+   * M_i is kept in one of three history slots of the workspace, slot i mod 3.  Draws no noise. */
+  const float *mq, *mr, *pm1, *pm2;   /* HOST tables [n_steps] (predictor == 2), else NULL */
 } b200_pc_config;
 
 B200_API int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b200_pc_t** out);

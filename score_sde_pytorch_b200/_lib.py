@@ -42,7 +42,8 @@ class PcConfig(ctypes.Structure):
               ('pa', P(c_float)), ('pb', P(c_float)), ('pc', P(c_float)),
               ('ca', P(c_float)), ('cb', P(c_float)), ('cc', P(c_float)),
               ('constraint', c_int), ('cm', P(c_float)), ('cs', P(c_float)),
-              ('color_m', c_float * 9), ('color_minv', c_float * 9), ('noise_nhwc', c_int)]
+              ('color_m', c_float * 9), ('color_minv', c_float * 9), ('noise_nhwc', c_int),
+              ('mq', P(c_float)), ('mr', P(c_float)), ('pm1', P(c_float)), ('pm2', P(c_float))]
 
 
 # name -> (restype, argtypes); must list every symbol declared in include/scoresde_b200.h

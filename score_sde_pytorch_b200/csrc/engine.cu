@@ -1973,14 +1973,23 @@ long long b200_ncsnpp_launches_per_forward(const b200_ncsnpp_t* h) { return h ? 
 // ===========================================================================
 // C ABI: predictor-corrector loop
 // ===========================================================================
-// per-step schedule tables of a PC plan (b200_pc_config: label .. cs); cm and cs only in constrained plans
-enum PcTable { PC_LABEL, PC_SS, PC_ALPHA, PC_PA, PC_PB, PC_PC, PC_CA, PC_CB, PC_CC, PC_CM, PC_CS, PC_TABLES };
+// per-step schedule tables of a PC plan (b200_pc_config: label .. cs, mq .. pm2); cm and cs only in constrained plans,
+// mq .. pm2 only in multistep plans (predictor == 2)
+enum PcTable { PC_LABEL, PC_SS, PC_ALPHA, PC_PA, PC_PB, PC_PC, PC_CA, PC_CB, PC_CC, PC_CM, PC_CS, PC_MQ, PC_MR, PC_PM1, PC_PM2,
+               PC_TABLES };
+
+static bool pc_table_used(const b200_pc_config& c, int k) {
+  if (k >= PC_MQ) return c.predictor == 2;
+  if (k >= PC_CM) return c.constraint != 0;
+  return true;
+}
 
 struct b200_pc {
   b200_ncsnpp* model; b200_pc_config cfg; int B; long long numel, per_img;
   std::vector<float> h_tab[PC_TABLES];   // host copies, uploaded by b200_pc_bind_workspace
   // workspace carve-up
   char* ws = nullptr; float* d_tab[PC_TABLES] = {}; float *labels, *net_out, *norms, *means;
+  float* hist = nullptr;   // multistep plans: three slots of numel floats (the last three data / noise predictions)
   int* d_step; unsigned long long* d_offset;
   PhiloxMap map;
   const float* known = nullptr; const float* mask = nullptr;   // constrained plans: bound by b200_pc_bind_constraint
@@ -1999,16 +2008,18 @@ long long pc_ws_layout(b200_pc* pc, char* base) {
   long long off = 0;
   auto take = [&](long long bytes) { long long o = off; off += (bytes + 255) & ~255LL; return base ? base + o : nullptr; };
   const int N = pc->cfg.n_steps;
-  for (int k = 0; k < PC_TABLES; ++k) if (k < PC_CM || pc->cfg.constraint) pc->d_tab[k] = (float*)take(N * 4LL);
+  for (int k = 0; k < PC_TABLES; ++k) if (pc_table_used(pc->cfg, k)) pc->d_tab[k] = (float*)take(N * 4LL);
   pc->labels = (float*)take(pc->B * 4LL); pc->net_out = (float*)take(pc->numel * 4LL);
   pc->norms = (float*)take(2LL * pc->B * 4); pc->means = (float*)take(256);
   pc->d_step = (int*)take(256); pc->d_offset = (unsigned long long*)take(256);
+  if (pc->cfg.predictor == 2) pc->hist = (float*)take(3 * pc->numel * 4LL);
   return off;
 }
 
-// randn_like calls per iteration: the corrector's inner steps, the predictor, and the two constraint blends
+// randn_like calls per iteration: the corrector's inner steps, the noisy predictor, and the two constraint blends
+// (the multistep ODE update draws none)
 unsigned long long pc_calls_per_step(const b200_pc_config& c) {
-  return (unsigned long long)((c.corrector ? c.n_corrector_steps : 0) + (c.predictor ? 1 : 0) + (c.constraint ? 2 : 0));
+  return (unsigned long long)((c.corrector ? c.n_corrector_steps : 0) + (c.predictor == 1 ? 1 : 0) + (c.constraint ? 2 : 0));
 }
 
 int pc_constrain(b200_pc* pc, float* x, float* x_mean, unsigned long long cps, unsigned long long call, cudaStream_t st) {
@@ -2026,6 +2037,12 @@ int pc_iteration(b200_pc* pc, float* x, float* x_mean, const float* noise_c, con
   PcStepScalars sc{t[PC_SS], t[PC_ALPHA], t[PC_PA], t[PC_PB], t[PC_PC]};
   const unsigned long long cps = pc_calls_per_step(c);
   if (int r = launch_fill_from_table(t[PC_LABEL], pc->d_step, pc->labels, pc->B, st)) return r;
+  if (c.predictor == 2) {
+    PcMultistepScalars ms{t[PC_MQ], t[PC_MR], t[PC_PA], t[PC_PB], t[PC_PM1], t[PC_PM2]};
+    if (int r = b200_ncsnpp_forward(m, x, pc->labels, 1, pc->net_out, st)) return r;
+    if (int r = launch_pc_multistep(x, x_mean, pc->net_out, pc->hist, pc->numel, pc->d_step, ms, st)) return r;
+    return launch_step_increment(pc->d_step, st);
+  }
   unsigned long long call = 0;
   if (c.corrector == 2) {
     // affine corrector (annealed Langevin dynamics, sampling.py:286-319): the step size is a per-step scalar, so the update is
@@ -2078,7 +2095,9 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   B200_REQUIRE(cfg->n_steps > 0 && cfg->label && cfg->pb, "pc_create: missing schedule tables");
   B200_REQUIRE(cfg->corrector >= 0 && cfg->corrector <= 2, "pc_create: corrector %d unsupported", cfg->corrector);
   B200_REQUIRE(cfg->corrector != 2 || (cfg->ca && cfg->cb && cfg->cc), "pc_create: affine corrector without its tables");
-  B200_REQUIRE(cfg->predictor == 0 || cfg->predictor == 1, "pc_create: predictor %d unsupported", cfg->predictor);
+  B200_REQUIRE(cfg->predictor >= 0 && cfg->predictor <= 2, "pc_create: predictor %d unsupported", cfg->predictor);
+  B200_REQUIRE(cfg->predictor != 2 || (cfg->corrector == 0 && cfg->constraint == 0),
+               "pc_create: the multistep ODE update (predictor 2) takes no corrector and no constraint");
   B200_REQUIRE(cfg->constraint >= 0 && cfg->constraint <= 2, "pc_create: constraint %d unsupported", cfg->constraint);
   B200_REQUIRE(!cfg->constraint || (cfg->cm && cfg->cs), "pc_create: constraint without its cm/cs tables");
   B200_REQUIRE(cfg->noise_nhwc == 0 || cfg->noise_nhwc == 1, "pc_create: noise_nhwc %d unsupported", cfg->noise_nhwc);
@@ -2092,10 +2111,12 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   const int N = cfg->n_steps;
   // a table the caller leaves null takes its default: label 0, score_scale 1, alpha 1, the predictor's and the
   // corrector's x_mean = 1 x + 0 out, x = x_mean + 0 z, and the constraint's marginal 1 known + 0 z
-  const float* src[PC_TABLES] = {cfg->label, cfg->score_scale, cfg->alpha, cfg->pa, cfg->pb, cfg->pc, cfg->ca, cfg->cb, cfg->cc, cfg->cm, cfg->cs};
-  const float dflt[PC_TABLES] = {0.f, 1.f, 1.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f, 1.f, 0.f};
+  // and the multistep update's M = 0 x + 1 out without history terms
+  const float* src[PC_TABLES] = {cfg->label, cfg->score_scale, cfg->alpha, cfg->pa, cfg->pb, cfg->pc, cfg->ca, cfg->cb, cfg->cc,
+                                 cfg->cm, cfg->cs, cfg->mq, cfg->mr, cfg->pm1, cfg->pm2};
+  const float dflt[PC_TABLES] = {0.f, 1.f, 1.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f, 1.f, 0.f, 0.f};
   for (int k = 0; k < PC_TABLES; ++k) {
-    if (k >= PC_CM && !cfg->constraint) continue;
+    if (!pc_table_used(*cfg, k)) continue;
     pc->h_tab[k].assign(N, dflt[k]);
     if (src[k]) memcpy(pc->h_tab[k].data(), src[k], N * 4);
   }
@@ -2105,6 +2126,7 @@ int b200_pc_create(b200_ncsnpp_t* model, const b200_pc_config* cfg, int batch, b
   }
   pc->cfg.label = pc->cfg.score_scale = pc->cfg.alpha = pc->cfg.pa = pc->cfg.pb = pc->cfg.pc = nullptr;
   pc->cfg.ca = pc->cfg.cb = pc->cfg.cc = pc->cfg.cm = pc->cfg.cs = nullptr;
+  pc->cfg.mq = pc->cfg.mr = pc->cfg.pm1 = pc->cfg.pm2 = nullptr;
   const long long cps = (cfg->corrector ? cfg->n_corrector_steps : 0) + (cfg->predictor ? 1 : 0);   // network evaluations
   const long long tail = cfg->constraint ? (cfg->predictor ? 1 : 0) + 2   /* predictor apply, two blends */
                                          : 1 /* predictor apply, or the x -> x_mean copy */;
@@ -2196,7 +2218,7 @@ int b200_pc_step_external(b200_pc_t* pc, float* x, float* x_mean, int step, cons
   PdlScope pdl(pc->model->cfg.pdl != 0);
   B200_REQUIRE(step >= 0 && step < pc->cfg.n_steps, "pc_step_external: step %d out of range", step);
   B200_REQUIRE(!pc->cfg.corrector || noise_c, "pc_step_external: corrector noise missing");
-  B200_REQUIRE(!pc->cfg.predictor || noise_p, "pc_step_external: predictor noise missing");
+  B200_REQUIRE(pc->cfg.predictor != 1 || noise_p, "pc_step_external: predictor noise missing");
   B200_REQUIRE(pc->cfg.n_corrector_steps <= 1 || !pc->cfg.corrector, "pc_step_external: supports n_steps_each <= 1");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   B200_CHECK_CUDA(cudaMemcpyAsync(pc->d_step, &step, 4, cudaMemcpyHostToDevice, st));

@@ -237,6 +237,13 @@ int launch_pc_constrain(float* x, float* x_mean, const float* known, const float
                         unsigned long long calls_per_step, unsigned long long call_idx,
                         const float* cm, const float* cs, const PcColorTransform& ct, int colorize, int C, long long HW,
                         cudaStream_t st);
+struct PcMultistepScalars {  // device tables of the multistep ODE update (b200_pc_config.predictor == 2)
+  const float *mq, *mr;      // M = mq*x + mr*out
+  const float *pa, *pb, *pm1, *pm2;   // x' = pa*x + pb*M + pm1*M_prev + pm2*M_prev2
+};
+// hist: three slots of numel floats; step s writes its M into slot s % 3 and reads M_{s-1}, M_{s-2} from the others
+int launch_pc_multistep(float* x, float* x_mean, const float* out, float* hist, long long numel, const int* step,
+                        PcMultistepScalars sc, cudaStream_t st);
 int launch_step_increment(int* step, cudaStream_t st);
 
 }  // namespace b200

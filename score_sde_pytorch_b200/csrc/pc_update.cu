@@ -243,6 +243,47 @@ __global__ void __launch_bounds__(256) pc_constrain_kernel(float* __restrict__ x
   }
 }
 
+// Multistep ODE update (b200_pc_config.predictor == 2), one element:  M = mq x + mr out,
+// x' = pa x + pb M (+ c1 M_prev) (+ c2 M_prev2), every product and sum rounded separately in this order, so an eager fp32
+// loop over the same tables reproduces it.  A zero coefficient skips its history term: the slots hold stale values
+// (or nothing yet) during the warm-up steps.
+__device__ __forceinline__ float multistep_elem(float x, float o, float* m0, const float* m1, const float* m2, float mq,
+                                                float mr, float pa, float pb, float c1, float c2) {
+  const float M = __fadd_rn(__fmul_rn(mq, x), __fmul_rn(mr, o));
+  *m0 = M;
+  float xn = __fadd_rn(__fmul_rn(pa, x), __fmul_rn(pb, M));
+  if (c1 != 0.f) xn = __fadd_rn(xn, __fmul_rn(c1, *m1));
+  if (c2 != 0.f) xn = __fadd_rn(xn, __fmul_rn(c2, *m2));
+  return xn;
+}
+
+__global__ void __launch_bounds__(256) pc_multistep_kernel(float* __restrict__ x, float* __restrict__ x_mean,
+                                                           const float* __restrict__ out, float* __restrict__ hist,
+                                                           long long numel, const int* __restrict__ step,
+                                                           PcMultistepScalars sc) {
+  pdl_wait(); pdl_trigger();   // programmatic dependent launch: see common.cuh
+  const int s = *step;
+  const float mq = sc.mq[s], mr = sc.mr[s], pa = sc.pa[s], pb = sc.pb[s], c1 = sc.pm1[s], c2 = sc.pm2[s];
+  float* h0 = hist + (long long)(s % 3) * numel;            // M_s
+  const float* h1 = hist + (long long)((s + 2) % 3) * numel; // M_{s-1}
+  const float* h2 = hist + (long long)((s + 1) % 3) * numel; // M_{s-2}
+  const long long n4 = numel >> 2;   // numel % 4 == 0 (launch_pc_multistep)
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 xv = reinterpret_cast<const float4*>(x)[i], ov = __ldg(reinterpret_cast<const float4*>(out) + i);
+    const float4 a = c1 != 0.f ? reinterpret_cast<const float4*>(h1)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 b = c2 != 0.f ? reinterpret_cast<const float4*>(h2)[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 m, r;
+    r.x = multistep_elem(xv.x, ov.x, &m.x, &a.x, &b.x, mq, mr, pa, pb, c1, c2);
+    r.y = multistep_elem(xv.y, ov.y, &m.y, &a.y, &b.y, mq, mr, pa, pb, c1, c2);
+    r.z = multistep_elem(xv.z, ov.z, &m.z, &a.z, &b.z, mq, mr, pa, pb, c1, c2);
+    r.w = multistep_elem(xv.w, ov.w, &m.w, &a.w, &b.w, mq, mr, pa, pb, c1, c2);
+    reinterpret_cast<float4*>(h0)[i] = m;
+    reinterpret_cast<float4*>(x)[i] = r;
+    if (x_mean) reinterpret_cast<float4*>(x_mean)[i] = r;
+  }
+}
+
 __global__ void step_increment_kernel(int* step) { pdl_wait(); pdl_trigger(); *step += 1; }
 
 int apply_grid(const PhiloxMap& m) {
@@ -305,6 +346,20 @@ int launch_pc_constrain(float* x, float* x_mean, const float* known, const float
   const int grid = (int)std::min<long long>((npix + 255) / 256, 132LL * 16);
   launch_kernel(pc_constrain_kernel, dim3(grid), dim3(256), 0, st, x, x_mean, known, mask, m, offset_dev, step,
                 calls_per_step, call_idx, cm, cs, ct, colorize, C, HW);
+  B200_CHECK_LAUNCH();
+  return 0;
+}
+
+int launch_pc_multistep(float* x, float* x_mean, const float* out, float* hist, long long numel, const int* step,
+                        PcMultistepScalars sc, cudaStream_t st) {
+  B200_REQUIRE(x && out && hist && step && sc.mq && sc.mr && sc.pa && sc.pb && sc.pm1 && sc.pm2,
+               "pc_multistep: null argument");
+  auto aligned = [](const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  B200_REQUIRE(aligned(x) && aligned(x_mean) && aligned(out) && aligned(hist) && numel % 4 == 0,
+               "pc_multistep: x, x_mean, out and hist must be 16-byte aligned with numel %% 4 == 0 (numel %lld)", numel);
+  if (numel == 0) return 0;
+  const int grid = (int)std::min<long long>((numel / 4 + 255) / 256, 132LL * 8);
+  launch_kernel(pc_multistep_kernel, dim3(grid), dim3(256), 0, st, x, x_mean, out, hist, numel, step, sc);
   B200_CHECK_LAUNCH();
   return 0;
 }

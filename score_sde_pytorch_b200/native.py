@@ -30,6 +30,10 @@ reference evaluates inside its loop, then handed to the C ABI as host arrays.
 :class:`ConstrainedPcPlan` for ``controllable_generation``: the same loop with
 the data-consistency blend (``controllable_generation.py:43-52`` / ``:137-146``)
 after the corrector block and after the predictor block of every iteration.
+
+``match_multistep_plan`` returns a :class:`MultistepPlan`: the same loop object running the multistep DPM-Solver /
+DPM-Solver++ update of the probability-flow ODE (``b200_pc_config.predictor = 2``) over the tables of
+:func:`build_multistep_tables`.
 """
 import ctypes
 
@@ -127,6 +131,7 @@ class PcPlan:
     self.predictor_kind, self.corrector_kind = predictor_kind, corrector_kind
     self.snr, self.n_steps, self.probability_flow, self.eps = float(snr), int(n_steps), bool(probability_flow), float(eps)
     self.tables = build_tables(sde, predictor_kind, corrector_kind, probability_flow, eps, snr=float(snr))
+    self.n_iters = sde.N           # iterations of the schedule (length of every table)
     self._pc = None
     self._ws = None
     self._engine_id = None
@@ -151,13 +156,13 @@ class PcPlan:
       return eng
     self._release()
     cfg = _lib.PcConfig()
-    cfg.n_steps = self.sde.N
+    cfg.n_steps = self.n_iters
     cfg.corrector = {'langevin': 1, 'ald': 2}.get(self.corrector_kind, 0)
     cfg.predictor = 0 if self.predictor_kind == 'none' else 1
     cfg.n_corrector_steps = self.n_steps
     cfg.snr = self.snr
     fp = ctypes.POINTER(ctypes.c_float)
-    for k in ('label', 'score_scale', 'alpha', 'pa', 'pb', 'pc', 'ca', 'cb', 'cc', 'cm', 'cs'):
+    for k in ('label', 'score_scale', 'alpha', 'pa', 'pb', 'pc', 'ca', 'cb', 'cc', 'cm', 'cs', 'mq', 'mr', 'pm1', 'pm2'):
       if k in self.tables:
         setattr(cfg, k, self.tables[k].ctypes.data_as(fp))
     self._configure(cfg)
@@ -191,7 +196,7 @@ class PcPlan:
     ``clone=False`` the plan's persistent buffers (overwritten by the next call)."""
     with torch.cuda.device(self.device):
       self._ensure()
-      num_steps = self.sde.N - first_step if num_steps is None else num_steps
+      num_steps = self.n_iters - first_step if num_steps is None else num_steps
       self._x.copy_(x.detach().reshape(self.shape), non_blocking=True)
       self._xm.copy_(self._x)
       x, x_mean = self._x, self._xm
@@ -258,6 +263,192 @@ class ConstrainedPcPlan(PcPlan):
       self._known.copy_(known.detach().expand(self.shape))
       self._mask.copy_(mask.detach().expand(self.shape))
       return super().run(x, first_step=first_step, num_steps=num_steps, clone=clone)
+
+
+MULTISTEP_ALGORITHMS = ('dpmsolver++', 'dpmsolver')
+MULTISTEP_SKIP_TYPES = ('logSNR', 'time_uniform', 'time_quadratic')
+
+
+def marginal_schedule(sde):
+  """``(log_alpha, log_sigma, t_of_lambda)`` of a stock SDE's Gaussian marginal ``x_t = alpha_t x_0 + sigma_t eps``, as
+  float64 numpy functions; ``lambda_t = log alpha_t - log sigma_t`` and ``t_of_lambda`` is its closed-form inverse.
+  ``sigma_t`` is the std ``models/utils.get_score_fn`` divides by (``sde.marginal_prob``), so ``eps = -sigma_t score``.
+
+  * VE: ``alpha_t = 1``, ``sigma_t = sigma_min (sigma_max / sigma_min)^t``: ``lambda`` is linear in ``t``.
+  * VP: ``log alpha_t = -(beta_1 - beta_0) t^2 / 4 - beta_0 t / 2``, ``sigma_t = sqrt(1 - alpha_t^2)``:
+    ``-log alpha = log1p(e^{-2 lambda}) / 2``.
+  * sub-VP: the same ``alpha_t``, ``sigma_t = 1 - alpha_t^2``: ``-log alpha = asinh(e^{-lambda} / 2)``.
+  For (sub-)VP ``t`` is then the positive root of the quadratic ``-log alpha_t = L``."""
+  if type(sde) not in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE):
+    raise NotImplementedError(f'SDE class {type(sde).__name__} has no closed-form log-SNR schedule: the multistep DPM-Solver '
+                              'samplers take VESDE, VPSDE and subVPSDE')
+  if isinstance(sde, sde_lib.VESDE):
+    lo, span = np.log(sde.sigma_min), np.log(sde.sigma_max) - np.log(sde.sigma_min)
+    return (lambda t: np.zeros_like(np.asarray(t, np.float64)), lambda t: lo + span * np.asarray(t, np.float64),
+            lambda lam: (-np.asarray(lam, np.float64) - lo) / span)
+  b0, d = float(sde.beta_0), float(sde.beta_1) - float(sde.beta_0)
+
+  def log_alpha(t):
+    t = np.asarray(t, np.float64)
+    return -0.25 * d * t ** 2 - 0.5 * b0 * t
+
+  if isinstance(sde, sde_lib.VPSDE):
+    log_sigma = lambda t: 0.5 * np.log(-np.expm1(2. * log_alpha(t)))
+    neg_log_alpha = lambda lam: 0.5 * np.logaddexp(0., -2. * np.asarray(lam, np.float64))
+  else:
+    log_sigma = lambda t: np.log(-np.expm1(2. * log_alpha(t)))
+    neg_log_alpha = lambda lam: np.arcsinh(0.5 * np.exp(-np.asarray(lam, np.float64)))
+
+  def t_of_lambda(lam):
+    L = neg_log_alpha(lam)
+    return 2. * L / (0.5 * b0 + np.sqrt(0.25 * b0 ** 2 + d * L))   # d/4 t^2 + b0/2 t - L = 0, cancellation-free
+
+  return log_alpha, log_sigma, t_of_lambda
+
+
+def multistep_orders(steps, order):
+  """Order of each step: ``min(order, i + 1)`` (warm-up: the history holds ``i + 1`` predictions); below 10 steps the
+  last steps also drop to ``min(order, steps - i)``, which keeps very short schedules stable."""
+  orders = [min(order, i + 1) for i in range(steps)]
+  if steps < 10:
+    orders = [min(o, steps - i) for i, o in enumerate(orders)]
+  return orders
+
+
+def multistep_coefficients(sde, t, orders, algorithm):
+  """float64 tables of the multistep update on the time grid ``t`` (``len(orders) + 1`` points, step ``i`` from
+  ``t[i]`` to ``t[i+1]`` at order ``orders[i]``), as ``M_i = mq_i x_i + ms_i score_i`` (``mr_i`` multiplies the network
+  output instead of the score) and ``x_{i+1} = pa_i x_i + pb_i M_i + pm1_i M_{i-1} + pm2_i M_{i-2}``.
+
+  ``M`` is the data prediction ``x0 = (x + sigma^2 score) / alpha`` for ``'dpmsolver++'`` and the noise prediction
+  ``eps = -sigma score`` for ``'dpmsolver'``.  With ``h = lambda_{i+1} - lambda_i``, the Taylor expansion of ``M`` in
+  ``lambda`` integrated exactly against the exponential weight gives (DPM-Solver++, arXiv:2211.01095, eq. 9;
+  DPM-Solver, arXiv:2206.00927, eq. 3.6; ``s = i``, ``t = i + 1``)
+
+    x0:  x_t = (sigma_t / sigma_s) x_s - alpha_t phi1 M - ... with phi1 = expm1(-h), phi2 = phi1 / h + 1, phi3 = phi2 / h - 1/2
+         and the terms +alpha_t phi2 (h M') and -alpha_t phi3 (h^2 M'')
+    eps: x_t = (alpha_t / alpha_s) x_s - sigma_t phi1 M - ... with phi1 = expm1(h), phi2 = phi1 / h - 1, phi3 = phi2 / h - 1/2
+         and the terms -sigma_t phi2 (h M') and -sigma_t phi3 (h^2 M'')
+
+  where ``h M'`` and ``h^2 M''`` come from divided differences of the stored predictions with the step ratios
+  ``r0 = (lambda_i - lambda_{i-1}) / h``, ``r1 = (lambda_{i-1} - lambda_{i-2}) / h``.  Order 2 is the paper's 2M form
+  ``A (M_i + (M_i - M_{i-1}) / (2 r0))``; order 1 is DDIM."""
+  log_alpha, log_sigma, _ = marginal_schedule(sde)
+  t = np.asarray(t, np.float64)
+  la, ls = log_alpha(t), log_sigma(t)
+  lam, alpha, sigma = la - ls, np.exp(la), np.exp(ls)
+  n = len(orders)
+  tab = {k: np.zeros(n) for k in ('pa', 'pb', 'pm1', 'pm2', 'mq', 'ms', 'mr')}
+  vp = not isinstance(sde, sde_lib.VESDE)
+  for i, k in enumerate(orders):
+    h = lam[i + 1] - lam[i]
+    if algorithm == 'dpmsolver++':
+      pa = np.exp(ls[i + 1] - ls[i])
+      phi1 = np.expm1(-h)
+      phi2 = phi1 / h + 1.
+      phi3 = phi2 / h - 0.5
+      A, B, C = -alpha[i + 1] * phi1, alpha[i + 1] * phi2, -alpha[i + 1] * phi3
+      mq, ms = 1. / alpha[i], sigma[i] ** 2 / alpha[i]
+    else:
+      pa = np.exp(la[i + 1] - la[i])
+      phi1 = np.expm1(h)
+      phi2 = phi1 / h - 1.
+      phi3 = phi2 / h - 0.5
+      A, B, C = -sigma[i + 1] * phi1, -sigma[i + 1] * phi2, -sigma[i + 1] * phi3
+      mq, ms = 0., -sigma[i]
+    c = [A, 0., 0.]
+    if k == 2:
+      r0 = (lam[i] - lam[i - 1]) / h
+      c = [A * (1. + 0.5 / r0), -0.5 * A / r0, 0.]
+    elif k == 3:
+      # D1_0 = (M_i - M_{i-1}) / r0, D1_1 = (M_{i-1} - M_{i-2}) / r1;  h M' = D1_0 + r0 (D1_0 - D1_1) / (r0 + r1) and
+      # h^2 M'' = 2 (D1_0 - D1_1) / (r0 + r1) to second order in h
+      r0, r1 = (lam[i] - lam[i - 1]) / h, (lam[i - 1] - lam[i - 2]) / h
+      c0 = B * (1. + r0 / (r0 + r1)) + 2. * C / (r0 + r1)   # coefficient of D1_0
+      c1 = -B * r0 / (r0 + r1) - 2. * C / (r0 + r1)         # coefficient of D1_1
+      c = [A + c0 / r0, -c0 / r0 + c1 / r1, -c1 / r1]
+    tab['pa'][i], tab['pb'][i], tab['pm1'][i], tab['pm2'][i] = pa, c[0], c[1], c[2]
+    tab['mq'][i], tab['ms'][i] = mq, ms
+    tab['mr'][i] = ms * (-1. / sigma[i] if vp else 1.)   # score = -out / sigma_t for (sub-)VP, out for VE
+  return tab
+
+
+def build_multistep_tables(sde, steps, order, algorithm='dpmsolver++', skip_type='logSNR', eps=1e-3):
+  """Per-step tables of the multistep DPM-Solver (``algorithm='dpmsolver'``) / DPM-Solver++ (``'dpmsolver++'``) sampler
+  of the probability-flow ODE: ``steps`` steps on ``steps + 1`` times from ``sde.T`` to ``eps``, uniform in log-SNR
+  ``lambda`` (``skip_type='logSNR'``), in ``t`` (``'time_uniform'``) or in ``sqrt(t)`` (``'time_quadratic'``).
+  Returns the float64 arrays of :func:`multistep_coefficients` plus ``t`` (``steps + 1``), ``orders`` and ``label``
+  (float32: the network time label at ``t[i]`` exactly as ``get_score_fn`` computes it for a float32 batch)."""
+  if order not in (1, 2, 3):
+    raise ValueError(f'order must be 1, 2 or 3, got {order!r}')
+  if not isinstance(steps, (int, np.integer)) or steps < 1:
+    raise ValueError(f'steps must be a positive integer, got {steps!r}')
+  if algorithm not in MULTISTEP_ALGORITHMS:
+    raise ValueError(f"algorithm must be one of {MULTISTEP_ALGORITHMS}, got {algorithm!r}")
+  if skip_type not in MULTISTEP_SKIP_TYPES:
+    raise ValueError(f"skip_type must be one of {MULTISTEP_SKIP_TYPES}, got {skip_type!r}")
+  log_alpha, log_sigma, t_of_lambda = marginal_schedule(sde)
+  T = float(sde.T)
+  if skip_type == 'logSNR':
+    lam = lambda v: log_alpha(v) - log_sigma(v)
+    t = t_of_lambda(np.linspace(lam(T), lam(eps), steps + 1))
+  elif skip_type == 'time_uniform':
+    t = np.linspace(T, eps, steps + 1)
+  else:
+    t = np.linspace(np.sqrt(T), np.sqrt(eps), steps + 1) ** 2
+  t[0], t[-1] = T, eps
+  orders = multistep_orders(int(steps), order)
+  tab = multistep_coefficients(sde, t, orders, algorithm)
+  t32 = torch.from_numpy(t[:-1]).to(torch.float32)
+  if isinstance(sde, sde_lib.VESDE):
+    label = sde.marginal_prob(torch.zeros(steps, 1, 1, 1), t32)[1]     # sigma(t), models/utils.py:164-165
+  else:
+    label = t32 * 999                                                  # models/utils.py:151
+  tab.update(t=t, orders=np.asarray(orders), label=np.ascontiguousarray(label.numpy().astype(np.float32)))
+  return tab
+
+
+class MultistepPlan(PcPlan):
+  """The native loop running the multistep DPM-Solver / DPM-Solver++ update (``b200_pc_config.predictor = 2``): per step
+  one network evaluation and one fused update kernel, replayed as a CUDA graph; no noise is drawn."""
+
+  def __init__(self, model, sde, shape, steps, order, algorithm, skip_type, eps, device):
+    self.model, self.sde, self.shape, self.device = model, sde, tuple(shape), model._explicit_device(device)
+    self.predictor_kind, self.corrector_kind = 'multistep', 'none'
+    self.snr, self.n_steps, self.probability_flow, self.eps = 0., 0, True, float(eps)
+    tab = build_multistep_tables(sde, steps, order, algorithm, skip_type, eps)
+    f32 = lambda v: np.ascontiguousarray(np.asarray(v, np.float64).astype(np.float32))
+    self.tables = {k: f32(tab[k]) for k in ('label', 'pa', 'pb', 'mq', 'mr', 'pm1', 'pm2')}
+    self.n_iters = int(steps)
+    self._pc = None
+    self._ws = None
+    self._engine_id = None
+    self._x = self._xm = None
+    self.use_graph = True
+
+  def _configure(self, cfg):
+    cfg.predictor, cfg.corrector = 2, 0
+
+
+def match_multistep_plan(sde, model, shape, steps, order, algorithm, skip_type, eps, device):
+  """Return a cached :class:`MultistepPlan` when ``model`` is an engine network taking time labels on a CUDA device and
+  ``sde`` a stock VE / VP / sub-VP SDE, else ``None`` (the caller runs the host loop)."""
+  from .models._engine import EngineModel
+  model = _unwrap(model)
+  if not isinstance(model, EngineModel) or torch.device(device).type != 'cuda' or not torch.cuda.is_available():
+    return None
+  if not model.takes_time_labels or type(sde) not in (sde_lib.VESDE, sde_lib.VPSDE, sde_lib.subVPSDE):
+    return None
+  sde_key = (type(sde).__name__,) + tuple(
+      float(getattr(sde, a)) for a in ('sigma_min', 'sigma_max', 'beta_0', 'beta_1') if hasattr(sde, a))
+  key = ('multistep', sde_key, int(steps), int(order), algorithm, skip_type, tuple(shape), float(eps),
+         str(model._explicit_device(device)))
+  cache = model.__dict__.setdefault('_pc_plans', {})
+  plan = cache.get(key)
+  if plan is None:
+    plan = MultistepPlan(model, sde, shape, steps, order, algorithm, skip_type, eps, device)
+    cache[key] = plan
+  return plan
 
 
 def _kind_of_predictor(predictor):

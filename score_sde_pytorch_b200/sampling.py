@@ -72,6 +72,13 @@ def get_sampling_fn(config, sde, shape, inverse_scaler, eps):
                           probability_flow=config.sampling.probability_flow,
                           continuous=config.training.continuous,
                           denoise=config.sampling.noise_removal, eps=eps, device=config.device)
+  if method == 'dpm_solver':
+    smp = config.sampling
+    return get_dpm_solver_sampler(sde=sde, shape=shape, inverse_scaler=inverse_scaler,
+                                  steps=getattr(smp, 'dpm_steps', 20), order=getattr(smp, 'dpm_order', 3),
+                                  algorithm=getattr(smp, 'dpm_algorithm', 'dpmsolver++'),
+                                  skip_type=getattr(smp, 'dpm_skip_type', 'logSNR'),
+                                  denoise=smp.noise_removal, eps=eps, device=config.device)
   raise ValueError(f"Sampler name {config.sampling.method} unknown.")
 
 
@@ -295,6 +302,14 @@ def get_pc_sampler(sde, shape, predictor, corrector, inverse_scaler, snr,
   return pc_sampler
 
 
+def _denoise_update(sde, model, x, eps):
+  """One reverse-diffusion predictor step at ``t = eps`` without noise: the ``noise_removal`` step of the ODE samplers
+  (``sampling.py:433-441``)."""
+  score_fn = get_score_fn(sde, model, train=False, continuous=True)
+  vec_eps = torch.ones(x.shape[0], device=x.device) * eps
+  return ReverseDiffusionPredictor(sde, score_fn, probability_flow=False).update_fn(x, vec_eps)[1]
+
+
 def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1e-5,
                     method='RK45', eps=1e-3, device='cuda', device_solver=None):
   """Probability-flow ODE sampler (``sampling.py:414-485``): same signature, same ``(samples, nfe)`` result.
@@ -309,9 +324,7 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
   records which solver ran and the method."""
 
   def denoise_update_fn(model, x):
-    score_fn = get_score_fn(sde, model, train=False, continuous=True)
-    vec_eps = torch.ones(x.shape[0], device=x.device) * eps
-    return ReverseDiffusionPredictor(sde, score_fn, probability_flow=False).update_fn(x, vec_eps)[1]
+    return _denoise_update(sde, model, x, eps)
 
   def drift_fn(model, x, t):
     score_fn = get_score_fn(sde, model, train=False, continuous=True)
@@ -369,3 +382,58 @@ def get_ode_sampler(sde, shape, inverse_scaler, denoise=False, rtol=1e-5, atol=1
       return inverse_scaler(x), nfe
 
   return ode_sampler
+
+
+def get_dpm_solver_sampler(sde, shape, inverse_scaler, steps=20, order=3, algorithm='dpmsolver++', skip_type='logSNR',
+                           denoise=False, eps=1e-3, device='cuda'):
+  """Multistep DPM-Solver (``algorithm='dpmsolver'``, noise prediction; Lu et al., arXiv:2206.00927) or DPM-Solver++
+  (``'dpmsolver++'``, data prediction; arXiv:2211.01095) sampler of the probability-flow ODE from ``sde.T`` to ``eps``:
+  ``steps`` network evaluations at ``order`` 1 (DDIM), 2 or 3 on a grid uniform in log-SNR (``skip_type='logSNR'``), in
+  ``t`` (``'time_uniform'``) or in ``sqrt(t)`` (``'time_quadratic'``); tables from :func:`native.build_multistep_tables`.
+  The network is evaluated as ``get_ode_sampler`` evaluates it (``get_score_fn(..., continuous=True)``) and ``denoise``
+  adds the same final ``noise_removal`` step (one more evaluation).
+
+  Returns ``sampler(model, z=None) -> (samples, nfe)``.  With an engine network that takes time labels on a CUDA device
+  the loop is native (one CUDA-graph replay per step: the forward and one fused update kernel); any other ``nn.Module``
+  runs an eager host loop over the same tables in the dtype of the state.  ``sampler.last_stats`` records ``loop``
+  (``'native'`` / ``'host'``), ``steps``, ``order`` and ``nfe``.  Raises ``ValueError`` for an ``order`` outside 1-3,
+  ``steps < 1`` or an unknown ``algorithm`` / ``skip_type``, and ``NotImplementedError`` for SDEs other than VESDE,
+  VPSDE and subVPSDE and for networks that take noise-level indices (NCSNv2)."""
+  from . import native
+  tab = native.build_multistep_tables(sde, steps, order, algorithm, skip_type, eps)
+
+  def host_loop(model, x):
+    score_fn = get_score_fn(sde, model, train=False, continuous=True)
+    prev = []                                   # M_{i-1}, M_{i-2}
+    for i in range(steps):
+      vec_t = torch.full((x.shape[0],), float(tab['t'][i]), dtype=x.dtype, device=x.device)
+      m = float(tab['mq'][i]) * x + float(tab['ms'][i]) * score_fn(x, vec_t)
+      xn = float(tab['pa'][i]) * x + float(tab['pb'][i]) * m
+      for c, mp in zip((tab['pm1'][i], tab['pm2'][i]), prev):
+        if c != 0:
+          xn = xn + float(c) * mp
+      prev = [m] + prev[:1]
+      x = xn
+    return x
+
+  def dpm_solver_sampler(model, z=None):
+    from .models._engine import EngineModel
+    net = native._unwrap(model)
+    if isinstance(net, EngineModel) and not net.takes_time_labels:
+      raise NotImplementedError(f'get_dpm_solver_sampler: {type(net).__name__} takes noise-level indices, not the '
+                                'continuous-time labels of the probability-flow ODE')
+    with torch.no_grad():
+      x = sde.prior_sampling(shape).to(device) if z is None else z
+      plan = native.match_multistep_plan(sde, model, shape, steps, order, algorithm, skip_type, eps, x.device) \
+          if x.is_cuda else None
+      if plan is not None:
+        x, _ = plan.run(x.to(torch.float32))
+      else:
+        x = host_loop(model, x)
+      nfe = steps + int(bool(denoise))
+      if denoise:
+        x = _denoise_update(sde, model, x, eps)
+      dpm_solver_sampler.last_stats = dict(loop='host' if plan is None else 'native', steps=steps, order=order, nfe=nfe)
+      return inverse_scaler(x), nfe
+
+  return dpm_solver_sampler
