@@ -121,6 +121,46 @@ B200_API int b200_gemm_nt_f32(const float* a, long long lda, int a_batch_rows, c
                               int w_batch_rows, int nbatch, int m, int n, int k, const float* bias,
                               int round_tf32, float* out, long long ldo, int impl, void* stream);
 
+/* ---- kernel tests: the contraction paths only the engine reaches ----------------------------------------------------
+ * One tensor-core contraction with every field the engine's planner can set: the fused GroupNorm quad sums, the NCHW
+ * network head (n_valid channels of a 128-row padded weight tile, / per_img_div[img * div_stride]), stride-2 VALID
+ * convolutions (input hin x win read with zero fill past its right / bottom edge), split-TF32 lo twins, per-image and
+ * image-independent row vectors, batched GEMMs with shared operands and pitches.  Fields mirror the library's internal
+ * contraction descriptor (csrc/kernels.h TcGemmDesc and Epilogue); store_mode is Epilogue::round_tf32 (0 fp32, 1 TF32
+ * grid, 2 fp16).  struct_bytes must equal sizeof(b200_tc_test_desc): a caller built against another layout is refused
+ * before anything is read.  The plan is created, launched once on `stream` and destroyed; its form ("swap-halo",
+ * "single256" ...) is copied into form (form_len bytes, NUL-terminated) when form is not NULL. */
+typedef struct {
+  int struct_bytes;
+  const void *a1, *a2; int c1, c2;                 /* A: NHWC sources (conv) or row-major [rows][a_ld] (gemm) */
+  int conv, h, w, nimg, taps, stride, valid_pad, hin, win, dilation, no_halo, f16;
+  long long a_rows, a_ld; int a_batch_rows;
+  const void* wt; int n_total, k_total; long long w_rows, w_ld; int w_batch_rows;   /* W: [tap][n_total][k_total] */
+  int nbatch, m_per_batch;
+  const void *a3, *a4; int c3, c4; const void* w2;  /* extra 1x1 phase (fused skip projection) */
+  int split; const void *a1_lo, *a2_lo, *a3_lo, *a4_lo, *w_lo, *w2_lo;
+  double* qstats;                                   /* [img][n_total/4][2], accumulated: zeroed by the caller */
+  const float* bias; const float* rowvec; long long rowvec_ld; const float* residual; long long ld_res;
+  const float* per_img_div; long long div_stride; float scale; int store_mode; int rows_per_img;
+  void* out; long long ld_out; int out_nchw; int n_valid;
+} b200_tc_test_desc;
+B200_API int b200_tc_contract_f32(const b200_tc_test_desc* d, char* form, int form_len, void* stream);
+/* The few-channel convolution (impl 3 of b200_conv_nhwc_f32) with GroupNorm(+SiLU) applied to its input on load, as the
+ * engine runs it: per-(image, channel) coefficients from the caller's fp64 quad sums q1 [batch][c1/4][2] and q2
+ * [batch][c2/4][2] (as b200_groupnorm_nhwc_f32 computes them) into coeff_ws (2 * batch * (c1 + c2) floats), then the
+ * convolution of the raw input x1 | x2.  qstats (optional, zeroed by the caller) receives the output's quad sums
+ * [batch][c_out/4][2]. */
+B200_API int b200_conv_lowc_gn_f32(const float* x1, int c1, const float* x2, int c2, int batch, int h, int w,
+                                   const float* w_packed, int c_out, int ksize, const double* q1, const double* q2,
+                                   const float* gamma, const float* beta, int groups, float eps, int silu, float* coeff_ws,
+                                   const float* bias, const float* rowvec, long long rowvec_ld, const float* residual,
+                                   float scale, int round_tf32, float* out, double* qstats, void* stream);
+/* The CUDA-core network head: out_nchw [batch][n][h][w] = (conv3x3(x; w) + bias) / div[img * div_stride] (div NULL: no
+ * division), n <= 4; x NHWC fp32, or fp16 elements when x_f16 (c % 64 == 0); w_packed [9][n][c] fp32. */
+B200_API int b200_head_small_n_f32(const void* x, int x_f16, int batch, int h, int w, int c, const float* w_packed,
+                                   const float* bias, int n, const float* div, long long div_stride, float* out_nchw,
+                                   void* stream);
+
 /* ---- NCSN++ score network ----------------------------------------------------
  * Replaces models/ncsnpp.py:38-381 (+ models/layerspp.py, models/layers.py:29-124,515-555,
  * models/up_or_down_sampling.py, op/) for configurations with Fourier embedding,

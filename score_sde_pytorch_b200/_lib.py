@@ -74,6 +74,12 @@ SIGNATURES = {
   'b200_pack_conv_weight_f32': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
   'b200_gemm_nt_f32': (c_int, [c_void_p, c_ll, c_int, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                c_int, c_void_p, c_ll, c_int, c_void_p]),
+  'b200_tc_contract_f32': (c_int, [c_void_p, c_char_p, c_int, c_void_p]),
+  'b200_conv_lowc_gn_f32': (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_ll,
+                                    c_void_p, c_float, c_int, c_void_p, c_void_p, c_void_p]),
+  'b200_head_small_n_f32': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_ll,
+                                    c_void_p, c_void_p]),
   'b200_ncsnpp_create': (c_int, [P(NcsnppConfig), P(c_void_p)]),
   'b200_ncsnpp_destroy': (None, [c_void_p]),
   'b200_ncsnpp_num_params': (c_int, [c_void_p]),

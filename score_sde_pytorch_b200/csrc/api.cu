@@ -236,4 +236,62 @@ int b200_gemm_nt_f32(const float* a, long long lda, int a_batch_rows, const floa
   return launch_conv_simt(s, st);
 }
 
+int b200_tc_contract_f32(const b200_tc_test_desc* t, char* form, int form_len, void* stream) {
+  B200_REQUIRE(t, "tc_contract: null descriptor");
+  B200_REQUIRE(t->struct_bytes == (int)sizeof(b200_tc_test_desc),
+               "tc_contract: descriptor of %d bytes, the library's b200_tc_test_desc has %d", t->struct_bytes,
+               (int)sizeof(b200_tc_test_desc));
+  auto f = [](const void* p) { return static_cast<const float*>(p); };
+  TcGemmDesc d; memset(&d, 0, sizeof(d));
+  d.a1 = f(t->a1); d.C1 = t->c1; d.a2 = f(t->a2); d.C2 = t->c2;
+  d.conv = t->conv; d.H = t->h; d.W = t->w; d.nimg = t->nimg; d.taps = t->taps; d.stride = t->stride;
+  d.valid_pad = t->valid_pad; d.Hin = t->hin; d.Win = t->win; d.dilation = t->dilation; d.no_halo = t->no_halo; d.f16 = t->f16;
+  d.a_rows = t->a_rows; d.a_ld = t->a_ld; d.a_batch_rows = t->a_batch_rows;
+  d.w = f(t->wt); d.N_total = t->n_total; d.K_total = t->k_total; d.w_rows = t->w_rows; d.w_ld = t->w_ld;
+  d.w_batch_rows = t->w_batch_rows; d.nbatch = t->nbatch; d.M_per_batch = t->m_per_batch;
+  d.a3 = f(t->a3); d.C3 = t->c3; d.a4 = f(t->a4); d.C4 = t->c4; d.w2 = f(t->w2);
+  d.split = t->split; d.a1_lo = f(t->a1_lo); d.a2_lo = f(t->a2_lo); d.a3_lo = f(t->a3_lo); d.a4_lo = f(t->a4_lo);
+  d.w_lo = f(t->w_lo); d.w2_lo = f(t->w2_lo);
+  d.qstats = t->qstats;
+  Epilogue& ep = d.epi;
+  ep.bias = t->bias; ep.rowvec = t->rowvec; ep.rowvec_ld = t->rowvec_ld; ep.residual = t->residual; ep.ld_res = t->ld_res;
+  ep.per_img_div = t->per_img_div; ep.div_stride = t->div_stride; ep.scale = t->scale; ep.round_tf32 = t->store_mode;
+  ep.rows_per_img = t->rows_per_img; ep.out = static_cast<float*>(t->out); ep.ld_out = t->ld_out; ep.out_nchw = t->out_nchw;
+  ep.n_valid = t->n_valid;
+  TcGemmPlan* pl = nullptr;
+  if (int r = tc_gemm_plan_create(d, &pl)) return r;
+  if (form && form_len > 0) { strncpy(form, tc_gemm_form(pl), form_len - 1); form[form_len - 1] = '\0'; }
+  const int r = tc_gemm_launch(pl, static_cast<cudaStream_t>(stream));
+  tc_gemm_plan_destroy(pl);
+  return r;
+}
+
+int b200_conv_lowc_gn_f32(const float* x1, int c1, const float* x2, int c2, int batch, int h, int w, const float* w_packed,
+                          int c_out, int ksize, const double* q1, const double* q2, const float* gamma, const float* beta,
+                          int groups, float eps, int silu, float* coeff_ws, const float* bias, const float* rowvec,
+                          long long rowvec_ld, const float* residual, float scale, int round_tf32, float* out, double* qstats,
+                          void* stream) {
+  B200_REQUIRE(x1 && w_packed && q1 && gamma && beta && coeff_ws && out, "conv_lowc_gn: null pointer");
+  B200_REQUIRE(ksize == 1 || ksize == 3, "conv_lowc_gn: ksize %d unsupported", ksize);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (!x2) c2 = 0;
+  float* gn_scale = coeff_ws;
+  float* gn_shift = coeff_ws + (long long)batch * (c1 + c2);
+  if (int r = launch_gn_coeff(c1, c2, q1, q2, gamma, beta, batch, h * w, groups, eps, gn_scale, gn_shift, st)) return r;
+  SimtConv s; memset(&s, 0, sizeof(s));
+  s.x1 = x1; s.C1 = c1; s.x2 = x2; s.C2 = c2; s.in_scale = 1.f; s.H = h; s.W = w; s.R = s.S = ksize; s.stride = 1;
+  s.pad = ksize / 2; s.OH = h; s.OW = w; s.nbatch = batch; s.a_batched = 1; s.w = w_packed; s.N = c_out;
+  s.gn_scale = gn_scale; s.gn_shift = gn_shift; s.gn_act = silu ? 1 : 0; s.qstats = qstats;
+  s.epi.bias = bias; s.epi.rowvec = rowvec; s.epi.rowvec_ld = rowvec_ld; s.epi.residual = residual; s.epi.ld_res = c_out;
+  s.epi.scale = scale; s.epi.round_tf32 = round_tf32; s.epi.rows_per_img = h * w; s.epi.out = out; s.epi.ld_out = c_out;
+  return launch_conv_lowc(s, st);
+}
+
+int b200_head_small_n_f32(const void* x, int x_f16, int batch, int h, int w, int c, const float* w_packed, const float* bias,
+                          int n, const float* div, long long div_stride, float* out_nchw, void* stream) {
+  B200_REQUIRE(x && w_packed && out_nchw, "head_small_n: null pointer");
+  return launch_conv3x3_small_n(static_cast<const float*>(x), w_packed, bias, div, div_stride, out_nchw, batch, h, w, c, n,
+                                x_f16, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

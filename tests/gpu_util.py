@@ -83,6 +83,40 @@ def gemm_nt(a, w, nbatch, m, n, k, lda=None, ldw=None, a_batch_rows=None, w_batc
   return out
 
 
+_vp, _i, _ll, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
+
+
+class TcTestDesc(ctypes.Structure):
+  """``b200_tc_test_desc`` (include/scoresde_b200.h); ``struct_bytes`` is filled in by ``tc_contract``."""
+  _fields_ = [('struct_bytes', _i),
+              ('a1', _vp), ('a2', _vp), ('c1', _i), ('c2', _i),
+              ('conv', _i), ('h', _i), ('w', _i), ('nimg', _i), ('taps', _i), ('stride', _i), ('valid_pad', _i),
+              ('hin', _i), ('win', _i), ('dilation', _i), ('no_halo', _i), ('f16', _i),
+              ('a_rows', _ll), ('a_ld', _ll), ('a_batch_rows', _i),
+              ('wt', _vp), ('n_total', _i), ('k_total', _i), ('w_rows', _ll), ('w_ld', _ll), ('w_batch_rows', _i),
+              ('nbatch', _i), ('m_per_batch', _i),
+              ('a3', _vp), ('a4', _vp), ('c3', _i), ('c4', _i), ('w2', _vp),
+              ('split', _i), ('a1_lo', _vp), ('a2_lo', _vp), ('a3_lo', _vp), ('a4_lo', _vp), ('w_lo', _vp), ('w2_lo', _vp),
+              ('qstats', _vp),
+              ('bias', _vp), ('rowvec', _vp), ('rowvec_ld', _ll), ('residual', _vp), ('ld_res', _ll),
+              ('per_img_div', _vp), ('div_stride', _ll), ('scale', _f), ('store_mode', _i), ('rows_per_img', _i),
+              ('out', _vp), ('ld_out', _ll), ('out_nchw', _i), ('n_valid', _i)]
+
+
+def tc_contract(device, struct_bytes=None, **fields):
+  """One tensor-core contraction through ``b200_tc_contract_f32``.  Tensor-valued fields are passed as device pointers,
+  the rest as given; returns the plan's form ("swap-halo", "single256", ...)."""
+  d = TcTestDesc()
+  d.struct_bytes = ctypes.sizeof(TcTestDesc) if struct_bytes is None else struct_bytes
+  d.scale = 1.0
+  for k, v in fields.items():
+    setattr(d, k, v.data_ptr() if isinstance(v, torch.Tensor) else v)
+  form = ctypes.create_string_buffer(64)
+  _lib.call('b200_tc_contract_f32', ctypes.byref(d), form, len(form),
+            _lib.stream_ptr(device) if device is not None else None)
+  return form.value.decode()
+
+
 def randn_like_torch(numel, seed, offset, device):
   out = torch.empty(numel, device=device, dtype=torch.float32)
   ws = torch.zeros(2, device=device, dtype=torch.int64)

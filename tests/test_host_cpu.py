@@ -218,6 +218,18 @@ def test_library_loads_and_exports_every_declared_symbol():
   assert isinstance(err, bytes)
 
 
+@pytest.mark.parametrize('delta', [-8, 8])
+def test_tc_contract_refuses_a_descriptor_of_another_size(delta):
+  """The ctypes mirror of b200_tc_test_desc must match the library's layout: a descriptor whose struct_bytes differs is
+  refused before any field is read (and before any device call, so this runs without a GPU)."""
+  import gpu_util
+  with pytest.raises(RuntimeError, match='descriptor of'):
+    gpu_util.tc_contract(None, struct_bytes=ctypes.sizeof(gpu_util.TcTestDesc) + delta)
+  # the mirror's own size is accepted: an empty descriptor gets as far as the shape check
+  with pytest.raises(RuntimeError, match='unsupported shape'):
+    gpu_util.tc_contract(None)
+
+
 def test_engine_param_table_matches_module_and_reference_names():
   for name in ('tiny', 'tiny_noattn', 'cifar10_ve'):
     cfg = golden_config(name)
